@@ -412,11 +412,6 @@ int gwb200_aligner_align_all(gwb200_aligner* a)
     P.skew          = 1;
     if (const char* e = std::getenv("GWB200_MYERS_SKEW")) // development A/B switch: 0 = classic score passes only
         P.skew = std::atoi(e) != 0 ? 1 : 0;
-    // both speculative passes in one warp (9 + 17 lanes at C4): the pass is bound by the dependent instruction stream of a lane,
-    // not by the two warps sharing issue slots, so this is off unless asked for
-    P.fuse = 0;
-    if (const char* e = std::getenv("GWB200_MYERS_FUSE")) // development A/B switch
-        P.fuse = std::atoi(e) != 0 ? 1 : 0;
     P.qpat          = a->qpat_d.p;
     P.qpat_elems    = qpat_el;
     P.slot_actions  = a->slot_actions_d.p;

@@ -66,7 +66,6 @@ struct DeviceParams
     int64_t ws_phys;             // 32-bit words one workspace really holds from its pv pointer on (pv | mv | score are contiguous)
     int32_t speculate;           // 1: two workspaces per CTA, the pass of the doubled estimate runs alongside (see the kernel)
     int32_t skew;                // 1: bands of >= 128 rows run the skewed score pass (myers_skew.cuh); 0: classic passes only (A/B)
-    int32_t fuse;                // 1: both speculative passes of an alignment in one warp when both are skewed passes (A/B)
     WordType* qpat;
     int32_t qpat_elems;          // elements per CTA (>= 4 * ceil(max_query/32))
     // per-alignment result slots: alignment i owns [seq_starts[2i], seq_starts[2i+2])
@@ -501,67 +500,6 @@ __device__ void compute_scores_skew(int32_t lane, const skew::Geom& g, uint4* __
             if (L.B <= g.last_block && cb >= 0 && cb < g.n_batches && skew::block_retired(g, L.B, cb))
             {
                 skew::lane_init(L, L.B + g.nbl); // the band has left the block: on to the next block of this lane
-                cb = s - L.B;
-            }
-            if (L.B <= g.last_block && cb >= 0 && cb < g.n_batches)
-            {
-                const int32_t t0  = skew::kK * cb;
-                const uint32_t tw = s_tgt[t0 >> 4] >> ((t0 & 15) * 2);
-                uint64_t eqs[skew::kK];
-#pragma unroll
-                for (int32_t k = 0; k < skew::kK; k++)
-                    eqs[k] = s_q64[((tw >> (2 * k)) & 3u) * kSkewQ64Stride + L.B];
-                uint64_t pm[skew::kK][2];
-                int32_t sc[skew::kK];
-                mine = skew::lane_step(g, L, cb, eqs, in, pm, sc);
-                if (skew::block_in_band(g, L.B, cb))
-                {
-#pragma unroll
-                for (int32_t k = 0; k < skew::kK; k++)
-                    dst[k * g.nbl] = make_uint4(static_cast<uint32_t>(pm[k][0]), static_cast<uint32_t>(pm[k][0] >> 32), static_cast<uint32_t>(pm[k][1]),
-                                                static_cast<uint32_t>(pm[k][1] >> 32));
-#pragma unroll
-                for (int32_t k = 0; k < skew::kK; k += 4)
-                    dst[(skew::kK + k / 4) * g.nbl] = make_uint4(static_cast<uint32_t>(sc[k]), static_cast<uint32_t>(sc[k + 1]),
-                                                                 static_cast<uint32_t>(sc[k + 2]), static_cast<uint32_t>(sc[k + 3]));
-                }
-            }
-        }
-    }
-    __syncwarp();
-}
-
-// Both speculative passes of an alignment in ONE warp: lanes [0, g0.nbl) run the pass of the current estimate, the next g1.nbl lanes
-// the pass of the doubled one (C4: 9 + 17 lanes). The passes have the same number of steps (same query and target); every lane
-// carries its own geometry. One warp per alignment on the schedulers instead of two competing for the same issue slots.
-__device__ void compute_scores_skew_pair(int32_t lane, const skew::Geom& g0, uint4* __restrict__ rec0, const skew::Geom& g1, uint4* __restrict__ rec1,
-                                         const uint64_t* s_q64, const uint32_t* s_tgt)
-{
-    const int32_t n_lanes = g0.nbl + g1.nbl;
-    if (lane < n_lanes)
-    {
-        const bool second   = lane >= g0.nbl;
-        const skew::Geom g  = second ? g1 : g0;
-        const int32_t ln    = second ? lane - g0.nbl : lane;
-        const int32_t first = second ? g0.nbl : 0;
-        const uint32_t mask = n_lanes == 32 ? kFull : ((1u << n_lanes) - 1u);
-        const int32_t up    = first + (ln + g.nbl - 1) % g.nbl;
-        skew::LaneState L;
-        skew::lane_init(L, ln);
-        skew::Link mine;
-        mine.hbits = 0;
-        mine.S0    = 0;
-        uint4* dst = (second ? rec1 : rec0) + ln;
-        const int32_t stride = skew::kChunks * g.nbl;
-        for (int32_t s = 0; s < g0.n_steps; ++s, dst += stride)
-        {
-            skew::Link in;
-            in.hbits   = __shfl_sync(mask, mine.hbits, up);
-            in.S0      = __shfl_sync(mask, mine.S0, up);
-            int32_t cb = s - L.B;
-            if (L.B <= g.last_block && cb >= 0 && cb < g.n_batches && skew::block_retired(g, L.B, cb))
-            {
-                skew::lane_init(L, L.B + g.nbl);
                 cb = s - L.B;
             }
             if (L.B <= g.last_block && cb >= 0 && cb < g.n_batches)
@@ -1309,41 +1247,7 @@ __global__ void __launch_bounds__(64, 8) myers_banded_kernel(const DeviceParams 
             const bool a_final = A.band_width == query_size || A.band_width == max_bandwidth;
             const bool run_b   = P.speculate && A.fits && !a_final && B.fits;
             const PassPlan& M  = (warp == 0) ? A : B;
-            // both passes in warp 0 when both take the skewed formulation and their blocks fit one warp
-            int32_t dbA = -1, deA = -1, dbB = -1, deB = -1;
-            bool fused = false;
-            if (P.fuse != 0 && run_b && skew_tables)
-            {
-                band_phases(A.band_width, query_size, target_size, A.p, dbA, deA);
-                band_phases(B.band_width, query_size, target_size, B.p, dbB, deB);
-                const skew::Geom GA = skew::make_geom(A.band_width, query_size, target_size, dbA);
-                const skew::Geom GB = skew::make_geom(B.band_width, query_size, target_size, dbB);
-                fused = skew::usable(GA) && skew::usable(GB) && GA.nbl + GB.nbl <= 32 && skew::words_needed(GA) <= P.ws_phys &&
-                        skew::words_needed(GB) <= P.ws_phys;
-                if (fused && warp == 0)
-                {
-                    uint4* recA = reinterpret_cast<uint4*>(P.pv + (static_cast<int64_t>(blockIdx.x) * 2) * P.ws_stride);
-                    uint4* recB = reinterpret_cast<uint4*>(P.pv + (static_cast<int64_t>(blockIdx.x) * 2 + 1) * P.ws_stride);
-                    compute_scores_skew_pair(lane, GA, recA, GB, recB, s_q64, s_tgt);
-                    __threadfence_block();
-                    const SkewGlobalLoader ldA{recA, &GA};
-                    const SkewGlobalLoader ldB{recB, &GB};
-                    const int32_t distA = skew::score_at(GA, A.band_width, target_size, ldA);
-                    const int32_t distB = skew::score_at(GB, B.band_width, target_size, ldB);
-                    if (lane == 0)
-                    {
-                        s_dist[0] = distA;
-                        s_dbeg[0] = dbA;
-                        s_dend[0] = deA;
-                        s_skew[0] = 1;
-                        s_dist[1] = distB;
-                        s_dbeg[1] = dbB;
-                        s_dend[1] = deB;
-                        s_skew[1] = 1;
-                    }
-                }
-            }
-            if (!fused && ((warp == 0 && A.fits) || (warp == 1 && run_b)))
+            if ((warp == 0 && A.fits) || (warp == 1 && run_b))
             {
                 pvm.rows = M.n_words_band;
                 mvm.rows = M.n_words_band;

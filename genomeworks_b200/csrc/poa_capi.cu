@@ -7,7 +7,7 @@
 #include "../../include/gwb200.h"
 #include "common.cuh"
 #include "poa_kernels.cuh"
-#include "poa_kernels_v2.cuh"
+#include "poa_kernels_tb.cuh"
 #include "poa_kernels_v3.cuh"
 
 #include <atomic>
@@ -39,6 +39,24 @@ bool use32bit_size(const gwb200_poa_config& c)
 {
     int32_t m = std::max(c.max_consensus_size, std::max(c.max_nodes_per_graph, c.matrix_sequence_dimension));
     return m > INT16_MAX;
+}
+
+// The kernel a batch launches (DESIGN.md 4.1)
+enum class PoaKernel
+{
+    tb, // poa_window_kernel_tb: the traceback band modes
+    v3, // poa_window_kernel_v3: every other mode up to the widest adaptive band
+    v1, // poa_window_kernel: wider bands and reads of 64 k bases and more
+};
+
+// The v3 kernel packs band starts in 16 bits; only the traceback kernel hosts the traceback-matrix alignment.
+PoaKernel select_kernel(const gwb200_poa_config& c)
+{
+    if (c.band_mode == GWB200_POA_STATIC_BAND_TRACEBACK || c.band_mode == GWB200_POA_ADAPTIVE_BAND_TRACEBACK)
+        return PoaKernel::tb;
+    if (c.alignment_band_width <= kMaxAdaptiveBW && c.max_sequence_size < 65536)
+        return PoaKernel::v3;
+    return PoaKernel::v1;
 }
 
 struct Carver
@@ -105,13 +123,9 @@ struct gwb200_poa_batch
     DeviceParams P{};
     V2Extra X{};
     V3Extra Y{};
-    bool use_v2 = true;
-    bool use_v3 = true;      // third-generation kernel (one warp per window, persistent grid); v2/v1 remain for the traceback band
-                             // modes, bands wider than 1536 and reads of 64 k bases and more
-    int32_t v3_ctas_per_sm = 0;
+    PoaKernel kernel = PoaKernel::v3;
     bool tb_mode = false;    // static_band_traceback / adaptive_band_traceback
     int32_t trace_bytes = 2; // sizeof(TraceT): 1 unless max_banded_pred_distance > 127 (cudapoa_limits.hpp:56-60)
-    int32_t nw_override = 0;
     bool timers_on = false;
     unsigned long long* d_timers = nullptr;
 
@@ -197,92 +211,44 @@ Sizes compute_sizes(const gwb200_poa_config& c, int32_t score_bytes, int32_t sz,
     return s;
 }
 
-// Kernel selection for a batch: warps per window and band chunks per warp (see DESIGN.md 4.1).
-struct V2Choice
-{
-    int32_t nw, maxc;
-};
-V2Choice choose_v2(const gwb200_poa_batch* b)
-{
-    if (b->tb_mode)
-        return {1, 1}; // the traceback-matrix alignment is a one-warp routine (poa_kernels_tb.cuh)
-    // warps per window: one per 128-column band chunk, at most 4; chunks per warp bounded by the widest band the mode can
-    // reach (adaptive bands grow up to 1536 = 12 chunks)
-    const bool adaptive   = b->cfg.band_mode == GWB200_POA_ADAPTIVE_BAND && b->cfg.alignment_band_width < kMaxAdaptiveBW;
-    const int32_t nchunks = adaptive ? kMaxAdaptiveBW / 128 : std::max(1, b->cfg.alignment_band_width / 128);
-    // up to 2 chunks one warp (no CTA barriers); wider bands use 4 warps
-    int32_t nw = nchunks >= 3 ? 4 : 1;
-    if (b->cfg.band_mode == GWB200_POA_FULL_BAND)
-        nw = 1;
-    if (b->nw_override > 0 && !adaptive && nchunks <= 4)
-        nw = b->nw_override; // development switch
-    if (b->nw_override > 0 && adaptive)
-        return b->nw_override == 1 ? V2Choice{1, 12} : (b->nw_override == 2 ? V2Choice{2, 6} : V2Choice{4, 3}); // development switch
-    if (nw == 1 && nchunks == 2)
-        return {1, 2};
-    if (nchunks > 4 || nw < std::min(nchunks, 4))
-        return {4, 3};
-    if (nw == 4)
-        return {4, 1};
-    if (nw == 2)
-        return {2, 1};
-    return {1, 1};
-}
-
-// Dynamic shared memory per CTA of the v2 kernel: the staged read (max_sequence_size + widest band) plus a ring of score rows;
-// the traceback tile and the topological-sort staging reuse it. Defaults: 31 KB (32-bit scores; 7 windows per SM for the
-// 4-warp kernels), 24 KB (16-bit scores), 12 KB (one-warp kernels with 16-bit scores, 16 per SM).
-// Reads longer than ~10 kb get a pool that holds the staged read plus two rows of the widest band (fewer resident windows,
-// which HBM capacity limits anyway at that size).
 // Dynamic shared memory per CTA of the v3 kernel. The resident windows of one SM share its 227 KB: the pool is what one CTA gets
 // when the batch's capacity (HBM) is spread over the SMs, at most 16 CTAs per SM (registers) -- a batch that HBM limits to a
 // few windows per SM gives each of them a deeper ring of score rows. Never less than two traceback tile buffers or two rows
 // of the widest band.
-int32_t v3_pool_bytes(gwb200_poa_batch* b)
+int32_t v3_pool_bytes(const gwb200_poa_batch* b)
 {
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, b->device_id);
     int smem_sm = 233472;
     cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, b->device_id);
-    int32_t ctas = static_cast<int32_t>(std::min<int64_t>(16, std::max<int64_t>(1, (static_cast<int64_t>(b->max_poas) + sms - 1) / sms)));
-    {
-        // 32-bit scores run their rows as a wavefront (poa_kernels_v4.cuh): 32 rows in flight per window need windows of
-        // 33 x (Wg x 20 + 20) bytes, Wg = 48 slots for the widest adaptive bands -> 6 windows per SM
-        const char* e = std::getenv("GWB200_POA_WAVEFRONT");
-        if (b->score32 && e && std::atoi(e) != 0)
-            ctas = std::min(ctas, 6);
-    }
-    if (const char* c = std::getenv("GWB200_POA_CTAS_PER_SM")) // development switch
-        ctas = std::max(1, std::min(32, std::atoi(c)));
-    if (const char* kb = std::getenv("GWB200_POA_POOL_KB")) // development switch
-    {
-        b->v3_ctas_per_sm = ctas;
-        return std::atoi(kb) * 1024;
-    }
+    const int32_t ctas    = static_cast<int32_t>(std::min<int64_t>(16, std::max<int64_t>(1, (static_cast<int64_t>(b->max_poas) + sms - 1) / sms)));
     const int64_t max_bw  = (b->cfg.band_mode == GWB200_POA_ADAPTIVE_BAND) ? kMaxAdaptiveBW : b->cfg.alignment_band_width;
     const int64_t need    = std::max<int64_t>(2 * (max_bw + 8) * b->score_bytes, 2 * (b->score32 ? TileBuf<int32_t>::kBytes : TileBuf<int16_t>::kBytes));
     const int64_t statics = sizeof(V3Shared) + 64;
     int64_t pool          = smem_sm / ctas - 1024 - statics;
     pool                  = std::min<int64_t>(pool, 96 * 1024) / 256 * 256;
     pool                  = std::max<int64_t>(pool, align_up64(need, 256));
-    b->v3_ctas_per_sm     = ctas;
     return static_cast<int32_t>(pool);
 }
 
-template <typename ScoreT, typename SizeT>
-int32_t v3_action(gwb200_poa_batch* b, int action)
+// Dynamic shared memory per CTA of the traceback-mode kernel, where the topological sort stages its counters and child words:
+// 24 KB (32-bit scores) or 12 KB (16-bit scores), so that up to 16 windows share an SM (__launch_bounds__(32, 16)). Batches of
+// long reads or wide bands get the size of the read plus two score rows of the band when that is larger (fewer resident
+// windows, which HBM capacity limits anyway at that size).
+int32_t tb_pool_bytes(const gwb200_poa_batch* b)
 {
-    // the wavefront rows (poa_kernels_v4.cuh, 32-bit scores) live in their own instantiation: its code and register budget
-    // do not weigh on the default kernel
-    auto kfn = poa_window_kernel_v3<ScoreT, SizeT, true, false>;
-    if (b->Y.use_bulk == 0)
-        kfn = poa_window_kernel_v3<ScoreT, SizeT, false, false>; // rows leave by per-lane vector stores (A/B switch GWB200_POA_BULK=0)
-    if constexpr (sizeof(ScoreT) == 4)
-    {
-        if (b->Y.wavefront != 0)
-            kfn = poa_window_kernel_v3<ScoreT, SizeT, true, true>;
-    }
-    const int32_t smem = b->X.pool_bytes;
+    const int64_t bw   = b->cfg.alignment_band_width;
+    const int64_t dflt = b->score32 ? 24 * 1024 : 12 * 1024;
+    const int64_t need = (b->cfg.max_sequence_size + bw + 24) + 2 * (bw + 8) * b->score_bytes;
+    return static_cast<int32_t>(std::max<int64_t>(dflt, align_up64(need, 1024)));
+}
+
+// Resident CTAs per SM of a one-warp kernel with `smem` bytes of dynamic shared memory, after making that pool size launchable.
+// The kernel's residency is sized against the full shared-memory carve-out; do not inherit a device-wide cache preference
+// another library set in this process (the reference does cudaDeviceSetCacheConfig(PreferL1), cudapoa_kernels.cuh:605).
+template <typename Kernel>
+int32_t pooled_occupancy(Kernel kfn, int32_t smem)
+{
     if (smem > 48 * 1024)
         cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaFuncSetAttribute(kfn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
@@ -292,113 +258,54 @@ int32_t v3_action(gwb200_poa_batch* b, int action)
         cudaGetLastError();
         nb = 0;
     }
-    if (action == 1)
-        return nb;
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, b->device_id);
-    const int32_t grid = std::max(1, std::min(b->poa_count, std::max(1, nb) * sms));
-    cudaMemsetAsync(b->Y.work_counter, 0, sizeof(int32_t), b->stream);
-    kfn<<<grid, 32, smem, b->stream>>>(b->P, b->X, b->Y);
-    return 0;
+    return nb;
 }
 
-int32_t v2_pool_bytes(const gwb200_poa_batch* b)
-{
-    const int64_t max_bw = (b->cfg.band_mode == GWB200_POA_ADAPTIVE_BAND) ? kMaxAdaptiveBW : b->cfg.alignment_band_width;
-    int64_t dflt         = b->score32 ? 31 * 1024 : 24 * 1024;
-    if (choose_v2(b).nw == 1)
-        dflt = b->score32 ? 24 * 1024 : 12 * 1024; // one-warp kernels (127 registers, __launch_bounds__(32, 16)): up to 16 windows per SM
-    const int64_t need   = (b->cfg.max_sequence_size + max_bw + 24) + 2 * (max_bw + 8) * b->score_bytes;
-    if (const char* kb = std::getenv("GWB200_POA_POOL_KB")) // development switch
-        return std::atoi(kb) * 1024;
-    return static_cast<int32_t>(std::max<int64_t>(dflt, align_up64(need, 1024)));
-}
-
-// action 0: launch; action 1: return resident CTAs per SM (occupancy) for the chosen kernel
-template <typename ScoreT, typename SizeT, int32_t NW, int32_t MAXC>
-int32_t v2_action(gwb200_poa_batch* b, int action)
-{
-    auto kfn           = poa_window_kernel_v2<ScoreT, SizeT, NW, MAXC>;
-    const int32_t smem = b->X.pool_bytes;
-    if (smem > 48 * 1024)
-        cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    // the kernel's residency is sized against the full shared-memory carve-out; do not inherit a device-wide cache preference
-    // another library set in this process (the reference does cudaDeviceSetCacheConfig(PreferL1), cudapoa_kernels.cuh:605)
-    cudaFuncSetAttribute(kfn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (action == 1)
-    {
-        int nb = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kfn, 32 * NW, smem) != cudaSuccess)
-        {
-            cudaGetLastError();
-            return 0;
-        }
-        return nb;
-    }
-    kfn<<<b->poa_count, 32 * NW, smem, b->stream>>>(b->P, b->X);
-    return 0;
-}
-
+// action 0: launch; action 1: return resident CTAs per SM (occupancy) of the batch's kernel
 template <typename ScoreT, typename SizeT>
 int32_t typed_action(gwb200_poa_batch* b, int action)
 {
-    if (b->use_v3)
+    if (b->kernel == PoaKernel::v1)
     {
-        if (action == 0)
+        if (action == 1)
         {
-            b->X.timers = b->timers_on ? b->d_timers : nullptr;
-            if (b->timers_on)
-                cudaMemsetAsync(b->d_timers, 0, sizeof(unsigned long long) * 8 * b->poa_count, b->stream);
+            int nb = 0;
+            auto kfn = poa_window_kernel<ScoreT, SizeT, false>;
+            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kfn, 32, 0) != cudaSuccess)
+            {
+                cudaGetLastError();
+                return 0;
+            }
+            return nb;
         }
-        const int32_t r = v3_action<ScoreT, SizeT>(b, action);
-        if (action == 0)
-            count_launch();
-        return r;
-    }
-    if (b->use_v2)
-    {
-        if (action == 0)
-        {
-            b->X.timers = b->timers_on ? b->d_timers : nullptr;
-            if (b->timers_on)
-                cudaMemsetAsync(b->d_timers, 0, sizeof(unsigned long long) * 8 * b->poa_count, b->stream);
-        }
-        const V2Choice ch = choose_v2(b);
-        int32_t r;
-        if (ch.nw == 1 && ch.maxc == 2)
-            r = v2_action<ScoreT, SizeT, 1, 2>(b, action);
-        else if (ch.nw == 1 && ch.maxc == 12)
-            r = v2_action<ScoreT, SizeT, 1, 12>(b, action);
-        else if (ch.nw == 2 && ch.maxc == 6)
-            r = v2_action<ScoreT, SizeT, 2, 6>(b, action);
-        else if (ch.nw == 4 && ch.maxc == 3)
-            r = v2_action<ScoreT, SizeT, 4, 3>(b, action);
-        else if (ch.nw == 4)
-            r = v2_action<ScoreT, SizeT, 4, 1>(b, action);
-        else if (ch.nw == 2)
-            r = v2_action<ScoreT, SizeT, 2, 1>(b, action);
+        dim3 grid(b->poa_count), block(32);
+        if (b->msa)
+            poa_window_kernel<ScoreT, SizeT, true><<<grid, block, 0, b->stream>>>(b->P);
         else
-            r = v2_action<ScoreT, SizeT, 1, 1>(b, action);
-        if (action == 0)
-            count_launch();
-        return r;
+            poa_window_kernel<ScoreT, SizeT, false><<<grid, block, 0, b->stream>>>(b->P);
+        count_launch();
+        return 0;
     }
+    const bool v3      = b->kernel == PoaKernel::v3;
+    const int32_t smem = b->X.pool_bytes;
+    const int32_t nb   = v3 ? pooled_occupancy(poa_window_kernel_v3<ScoreT, SizeT>, smem) : pooled_occupancy(poa_window_kernel_tb<ScoreT, SizeT>, smem);
     if (action == 1)
-    {
-        int nb = 0;
-        auto kfn = poa_window_kernel<ScoreT, SizeT, false>;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kfn, 32, 0) != cudaSuccess)
-        {
-            cudaGetLastError();
-            return 0;
-        }
         return nb;
+    b->X.timers = b->timers_on ? b->d_timers : nullptr;
+    if (b->timers_on)
+        cudaMemsetAsync(b->d_timers, 0, sizeof(unsigned long long) * 8 * b->poa_count, b->stream);
+    if (v3)
+    {
+        int sms = 132;
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, b->device_id);
+        const int32_t grid = std::max(1, std::min(b->poa_count, std::max(1, nb) * sms));
+        cudaMemsetAsync(b->Y.work_counter, 0, sizeof(int32_t), b->stream);
+        poa_window_kernel_v3<ScoreT, SizeT><<<grid, 32, smem, b->stream>>>(b->P, b->X, b->Y);
     }
-    dim3 grid(b->poa_count), block(32);
-    if (b->msa)
-        poa_window_kernel<ScoreT, SizeT, true><<<grid, block, 0, b->stream>>>(b->P);
     else
-        poa_window_kernel<ScoreT, SizeT, false><<<grid, block, 0, b->stream>>>(b->P);
+    {
+        poa_window_kernel_tb<ScoreT, SizeT><<<b->poa_count, 32, smem, b->stream>>>(b->P, b->X);
+    }
     count_launch();
     return 0;
 }
@@ -659,10 +566,7 @@ static int poa_batch_create_impl(gwb200_poa_batch** out, int32_t device_id, void
         return set_error(GWB200_E_INVALID_ARGUMENT, "max_banded_pred_distance has to be positive in the traceback band modes");
     }
     b->bid              = gwb200_poa_batch::batches++;
-    {
-        const char* nwv = std::getenv("GWB200_POA_WARPS"); // development switch: warps per window (1, 2 or 4)
-        b->nw_override  = nwv ? std::atoi(nwv) : 0;
-    }
+    b->kernel           = select_kernel(*cfg);
 
     size_t free_b = 0, total_b = 0;
     if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess)
@@ -795,7 +699,6 @@ static int poa_batch_create_impl(gwb200_poa_batch** out, int32_t device_id, void
         b->d_timers      = dc.take<unsigned long long>(n * 8);
         b->Y.work_counter = dc.take<int32_t>(64);
         b->X.timers      = nullptr;
-        b->X.pool_bytes  = v2_pool_bytes(b);
         b->X.tb_scores   = nullptr;
         b->X.tb_trace    = nullptr;
         b->X.tb_height   = cfg->max_banded_pred_distance;
@@ -828,36 +731,13 @@ static int poa_batch_create_impl(gwb200_poa_batch** out, int32_t device_id, void
     }
     cudaEventCreate(&b->ev0);
     cudaEventCreate(&b->ev1);
+    if (b->kernel == PoaKernel::v3)
     {
-        const char* k = std::getenv("GWB200_POA_KERNEL"); // development A/B switch: "v1" / "v2" select the earlier kernel generations
-        b->use_v2     = !(k && std::string(k) == "v1");
-        b->use_v3     = !(k && (std::string(k) == "v1" || std::string(k) == "v2"));
-        {
-            // the v2 kernel packs band starts in 15 bits (x4) and needs its staged read plus a few score rows in shared memory
-            if (b->cfg.alignment_band_width > kMaxAdaptiveBW || b->cfg.max_sequence_size >= 65536 || b->X.pool_bytes > 200 * 1024)
-                b->use_v2 = false; // first-generation kernel
-            if (b->tb_mode)
-                b->use_v2 = true; // only the v2 kernel family hosts the traceback-matrix alignment
-            // the v3 kernel packs band starts in 16 bits and serves every score-matrix mode; the traceback-matrix modes stay on v2
-            if (b->cfg.alignment_band_width > kMaxAdaptiveBW || b->cfg.max_sequence_size >= 65536 || b->tb_mode)
-                b->use_v3 = false;
-        }
-        if (b->use_v3)
-        {
-            b->X.pool_bytes = v3_pool_bytes(b);
-            const char* e   = std::getenv("GWB200_POA_BULK"); // development A/B switches
-            b->Y.use_bulk   = (e && std::atoi(e) == 0) ? 0 : 1;
-            e               = std::getenv("GWB200_POA_TB_TMA");
-            b->Y.tb_tma     = (e && std::atoi(e) == 0) ? 0 : 1;
-            e               = std::getenv("GWB200_POA_GROUP"); // development switch: chunks per straight-line group (4, 2, 1)
-            // 32-bit scores: 8 cells per lane and chunk, groups of one chunk (8 cells per lane in flight)
-            b->Y.max_group  = e ? std::atoi(e) : (b->score32 ? 1 : 2);
-            e               = std::getenv("GWB200_POA_ROW_FENCE"); // development A/B switch: 1 = proxy fence in front of every general row
-            b->Y.row_fence  = (e && std::atoi(e) != 0) ? 1 : 0;
-            e               = std::getenv("GWB200_POA_WAVEFRONT");
-            b->Y.wavefront  = (e && std::atoi(e) != 0) ? 1 : 0; // off by default until it beats dp_rows_v3 (development switch)
-        }
+        b->X.pool_bytes = v3_pool_bytes(b);
+        b->Y.max_group32 = 1;
     }
+    else if (b->kernel == PoaKernel::tb)
+        b->X.pool_bytes = tb_pool_bytes(b);
     gwb200_poa_batch_reset(b);
     *out = b;
     return 0;

@@ -1,39 +1,23 @@
-// gw-b200 POA device code, second generation (sm_90a). Same behavioural contract as poa_kernels.cuh (identical
-// consensus / coverage / MSA / status to the reference kernels), restructured so that no phase stalls on dependent global
-// loads:
+// gw-b200 POA device code (sm_90a): the one-warp phases that the v3 kernel (poa_kernels_v3.cuh) and the traceback-mode kernel
+// (poa_kernels_tb.cuh) share, with the same behavioural contract as poa_kernels.cuh (identical consensus / coverage / MSA /
+// status to the reference kernels).
 //
-//   DP rows      the CTA has up to 4 warps, band chunk c (128 columns, 4 cells per lane) belongs to warp c % NW and only
-//                min(NW, chunks) warps take part in an alignment's rows (named barrier); per-row graph metadata (node, base,
-//                predecessor rows and band starts, ring distances, sink flag) is fetched 32 rows at a time by the lanes, one
-//                group ahead of its use, packed into three words and broadcast by three shuffles; the last R score rows live
-//                in a shared-memory ring so predecessor rows are read from shared memory, not L2/HBM; chunk carries are
-//                exchanged through shared memory and folded by one redux.sync.max per chunk; each row is written to HBM
-//                exactly once with aligned vector stores (the algorithmic sizeof(ScoreT) bytes per cell).
-//   end cell     lane-parallel over the sink rows.
-//   traceback    warp-uniform walk over a shared-memory tile (32 rows x 64 columns of scores + the rows' metadata)
-//                that the warp refills with coalesced loads; the reference's per-step preference order
-//                (cudapoa_nw_banded.cuh:440-534) and adaptive-band abort tests are evaluated unchanged on tile values;
-//                runs of "diagonal through the first predecessor" are taken 32 steps at a time (pointer doubling over the
-//                tile's first-predecessor links, lane k verifies step k).
 //   add alignment lane-parallel over read bases (new-node ids by ballot prefix sum); conflict-free because a path
 //                visits every node, ring and edge at most once.
 //   topsort      same Kahn FIFO order (cudapoa_topsort.cuh:45-97): in-degree counters, a tagged window of the FIFO and as
 //                many "only child" words as fit live in shared memory; single-child chains are followed in a register.
-//   traceback band modes: poa_kernels_tb.cuh (one-warp routine hosted by the NW = 1 instantiation).
+//
+// Also the per-batch kernel arguments (V2Extra), the phase timers and small score-row helpers.
 #pragma once
 #include <type_traits>
 
 #include "poa_kernels.cuh"
-#include "poa_kernels_tb.cuh"
 
 namespace gwb200
 {
 namespace poa
 {
 
-#ifndef GWB200_POA_NW4_BLOCKS
-#define GWB200_POA_NW4_BLOCKS 7 // resident windows per SM the 4-warp kernels are compiled for (register budget)
-#endif
 constexpr int32_t kTileRows = 32;
 constexpr int32_t kTileCols = 64;
 
@@ -81,749 +65,6 @@ template <typename ScoreT>
 __device__ __noinline__ int32_t band_get_slow(const Band<ScoreT>& B, int32_t row, int32_t column)
 {
     return B.get(row, column);
-}
-
-// needlemanWunschBanded (cudapoa_nw_banded.cuh:177-557), v2. The CTA has NW warps: the DP rows are computed by all of them
-// (band chunk c of 128 columns belongs to warp c % NW, carries between chunks are combined through shared memory with the
-// same max-plus algebra the in-warp scan uses); end-cell search and traceback run on warp 0. Returns the same value on
-// every thread.
-template <typename ScoreT, typename SizeT, int32_t NW, int32_t MAXC>
-__device__ int32_t nw_banded_v2(const Win<SizeT>& g, int32_t graph_count, const uint8_t* read, int32_t read_length, ScoreT* scores,
-                                float max_buffer_size, SizeT* aln_graph, SizeT* aln_read, int32_t band_width, int32_t gap, int32_t mismatch,
-                                int32_t match, int32_t rerun, const bool Adaptive, unsigned long long& cells, int4* row_meta, uint8_t* pool,
-                                int32_t pool_bytes, unsigned long long* timers, int32_t* s_xchg)
-{
-    constexpr int32_t kMin    = min_score_of<ScoreT>();
-    constexpr int32_t kNegInf = -(1 << 30); // "no carry-in" for the chunk-local closure (int32 arithmetic, cannot overflow)
-    constexpr int32_t kMaxChunksPerWarp = MAXC;
-    const int32_t lane = threadIdx.x & 31;
-    const int32_t warp = threadIdx.x >> 5;
-    GWB200_TIMER_START();
-
-    const float gradient     = __fdividef(static_cast<float>(read_length + 1), static_cast<float>(graph_count + 1));
-    const int32_t max_column = read_length + 1;
-    if (Adaptive)
-    {
-        if (static_cast<double>(gradient) > 1.1)
-        {
-            int32_t v  = static_cast<int32_t>(max_column * 0.08 * static_cast<double>(gradient));
-            band_width = max(band_width, (v + kMinBandWidth - 1) & ~(kMinBandWidth - 1));
-        }
-        if (static_cast<double>(gradient) < 0.8)
-        {
-            int32_t v  = static_cast<int32_t>(max_column * 0.1 / static_cast<double>(gradient));
-            band_width = max(band_width, (v + kMinBandWidth - 1) & ~(kMinBandWidth - 1));
-        }
-        band_width = min(band_width, kMaxAdaptiveBW);
-        if (band_width == kMaxAdaptiveBW && rerun != 0)
-            return rerun;
-    }
-    int32_t band_shift = band_width / 2;
-    if (Adaptive)
-    {
-        if (rerun == kShiftLeft && band_width <= kMaxAdaptiveBW / 2)
-        {
-            band_width *= 2;
-            band_shift = static_cast<int32_t>(band_shift * 2.5);
-        }
-        if (rerun == kShiftRight && band_width <= kMaxAdaptiveBW / 2)
-        {
-            band_width *= 2;
-            band_shift = static_cast<int32_t>(band_shift * 1.5);
-        }
-        const float required = static_cast<float>(graph_count) * static_cast<float>(band_width + kRightPad);
-        if (required > max_buffer_size)
-            return kNWStorageFail;
-    }
-    if (threadIdx.x == 0)
-        cells += static_cast<unsigned long long>(graph_count) * static_cast<unsigned long long>(band_width);
-
-    Band<ScoreT> B{scores, band_width, band_shift, max_column, band_width + kRightPad, gradient};
-    const int32_t stride = B.stride;
-    const int32_t nchunks = band_width / 128;
-    // warps that take part in the DP rows of this alignment: one per chunk, at most NW; warps without a chunk skip the rows
-    // (and their per-row preamble) and wait at the barrier after them
-    const int32_t nw_eff = min(NW, nchunks);
-    auto row_sync = [&]() {
-        if (NW == 1 || nw_eff == 1)
-            __syncwarp();
-        else
-            asm volatile("bar.sync 1, %0;" ::"r"(32 * nw_eff) : "memory");
-    };
-
-    // ---- shared memory during the DP phase: [ staged read | ring of the most recent score rows (row r in slot r % R) ]
-    const int32_t sread_bytes = (read_length + band_width + 8 + 15) & ~15;
-    uint8_t* sread            = pool;
-    ScoreT* ring              = reinterpret_cast<ScoreT*>(pool + sread_bytes);
-    int32_t R                 = (pool_bytes - sread_bytes) / (stride * static_cast<int32_t>(sizeof(ScoreT)));
-    R                         = min(R, 64);
-    const bool use_ring       = R >= 2;
-    if (R < 1)
-        R = 1;
-    {
-        // stage the read (4-byte aligned in the packed input); bytes past its end are zero: they only ever reach cells with
-        // column > read_length, which never influence columns <= read_length
-        const uint32_t* rd32 = reinterpret_cast<const uint32_t*>(read);
-        uint32_t* sr32       = reinterpret_cast<uint32_t*>(sread);
-        const int32_t nfull  = read_length >> 2;
-        for (int32_t i = threadIdx.x; i < sread_bytes / 4; i += 32 * NW)
-        {
-            uint32_t v = 0;
-            if (i < nfull)
-                v = __ldg(rd32 + i);
-            else if (i == nfull && (read_length & 3))
-                v = __ldg(rd32 + i) & ((1u << (8 * (read_length & 3))) - 1u);
-            sr32[i] = v;
-        }
-    }
-    for (int32_t j = threadIdx.x; j < stride; j += 32 * NW)
-    {
-        const ScoreT v = static_cast<ScoreT>(j * gap);
-        scores[j]      = v;
-        if (use_ring)
-            ring[j] = v;
-    }
-    __syncthreads();
-
-    // ---- per-row metadata: fetched 32 rows at a time by the lanes, one group ahead of its use (every warp keeps its own
-    // copy, the loads hit L1); warp 0 also writes it to row_meta for the end-cell search and the traceback.
-    // packed per-row words (broadcast by three shuffles per row):
-    //   misc: base | in-degree << 8 | sink << 16 | (band start / 4) << 17        (also what row_meta.w holds)
-    //   w1  : band start of predecessor 0 | band start of predecessor 1 << 16
-    //   w2  : min(row - pred0 row, 255) | min(row - pred1 row, 255) << 8 | "both predecessors are in the ring" << 16
-    int32_t nx_node = 0, nx_misc = 0, nx_p0 = 0, nx_p1 = 0, nx_w1 = 0, nx_w2 = 0;
-    auto pack_row = [&](int32_t row, int32_t node, int32_t base, int32_t pc, int32_t oc, int32_t e0, int32_t e1) {
-        nx_node           = node;
-        nx_p0             = pc > 0 ? static_cast<int32_t>(g.pos[e0]) + 1 : 0;
-        nx_p1             = pc > 1 ? static_cast<int32_t>(g.pos[e1]) + 1 : 0;
-        nx_misc           = base | (pc << 8) | ((oc == 0 ? 1 : 0) << 16) | ((B.start(row) >> 2) << 17);
-        nx_w1             = B.start(nx_p0) | (B.start(nx_p1) << 16);
-        const int32_t d0  = min(row - nx_p0, 255);
-        const int32_t d1  = min(row - nx_p1, 255);
-        const bool inring = use_ring && pc <= 2 && d0 < R && (pc < 2 || d1 < R);
-        nx_w2             = d0 | (d1 << 8) | ((inring ? 1 : 0) << 16);
-    };
-    {
-        const int32_t row = 1 + lane;
-        if (row <= graph_count)
-        {
-            const int32_t node = g.sorted[row - 1];
-            pack_row(row, node, g.nodes[node], g.in_cnt[node], g.out_cnt[node], g.in_edge(node, 0), g.in_edge(node, 1));
-        }
-    }
-#ifdef GWB200_ROW_PROFILE
-    unsigned long long rp_a = 0, rp_b = 0;
-#endif
-    int32_t ring_slot = 0; // slot of the current row = row % R, maintained incrementally
-    ScoreT* rowp      = scores; // row pointer in global memory, bumped once per row
-    const int32_t G   = 128 * gap;
-
-    for (int32_t r0 = 1; r0 <= graph_count && warp < nw_eff; r0 += 32)
-    {
-        const int32_t cur_node = nx_node, cur_misc = nx_misc, cur_p0 = nx_p0, cur_p1 = nx_p1, cur_w1 = nx_w1, cur_w2 = nx_w2;
-        const int32_t nrows    = min(32, graph_count - r0 + 1);
-        const bool have_next   = r0 + 32 <= graph_count;
-        if (warp == 0 && lane < nrows)
-            row_meta[r0 + lane] = make_int4(cur_node, cur_p0, cur_p1, cur_misc);
-        const int32_t nrow = r0 + 32 + lane;
-        const bool nvalid  = have_next && nrow <= graph_count;
-        int32_t t_node = 0, t_base = 0, t_pc = 0, t_oc = 1, t_e0 = 0, t_e1 = 0;
-
-        for (int32_t k = 0; k < nrows; k++)
-        {
-            if (have_next)
-            {
-                if (k == 0)
-                {
-                    if (nvalid)
-                        t_node = g.sorted[nrow - 1];
-                }
-                else if (k == 10)
-                {
-                    if (nvalid)
-                    {
-                        t_base = g.nodes[t_node];
-                        t_pc   = g.in_cnt[t_node];
-                        t_oc   = g.out_cnt[t_node];
-                        t_e0   = g.in_edge(t_node, 0);
-                        t_e1   = g.in_edge(t_node, 1);
-                    }
-                }
-                else if (k == 20)
-                {
-                    if (nvalid)
-                    {
-                        pack_row(nrow, t_node, t_base, t_pc, t_oc, t_e0, t_e1);
-                    }
-                }
-            }
-#ifdef GWB200_ROW_PROFILE
-            const unsigned long long rp_t0 = clock64();
-#endif
-            const int32_t row  = r0 + k;
-            const int32_t misc = __shfl_sync(kFull, cur_misc, k);
-            const int32_t w1   = __shfl_sync(kFull, cur_w1, k);
-            const int32_t w2   = __shfl_sync(kFull, cur_w2, k);
-            const int32_t base = misc & 0xff;
-            const int32_t pc   = (misc >> 8) & 0xff;
-            const int32_t bs   = ((misc >> 17) & 0x3fff) << 2;
-            const int32_t bsp0 = w1 & 0xffff;
-            ring_slot          = (ring_slot + 1 == R) ? 0 : ring_slot + 1;
-            rowp += stride;
-            ScoreT* srow       = ring + ring_slot * stride;
-            int32_t* xchg      = s_xchg + (row & 1) * 16; // chunk-out values, double buffered by row parity
-
-            int32_t local0, carry0;
-            int32_t a0[kMaxChunksPerWarp], a1[kMaxChunksPerWarp], a2[kMaxChunksPerWarp], a3[kMaxChunksPerWarp];
-            if (w2 & 0x10000)
-            {
-                // ---- common case: at most two predecessors, both still in the shared-memory ring
-                int32_t sl0 = ring_slot - (w2 & 0xff);
-                if (sl0 < 0)
-                    sl0 += R;
-                const ScoreT* prow0 = ring + sl0 * stride;
-                const int32_t bep0  = min(bsp0 + band_width - kCPT, max_column);
-                const ScoreT* prow1 = prow0;
-                int32_t bsp1 = 0, bep1 = -1;
-                if (pc == 2)
-                {
-                    int32_t sl1 = ring_slot - ((w2 >> 8) & 0xff);
-                    if (sl1 < 0)
-                        sl1 += R;
-                    prow1 = ring + sl1 * stride;
-                    bsp1  = static_cast<int32_t>(static_cast<uint32_t>(w1) >> 16);
-                    bep1  = min(bsp1 + band_width - kCPT, max_column);
-                }
-                int32_t first = 0;
-                if (pc != 0)
-                {
-                    if (bs > kCPT && pc == 1)
-                    {
-                        first = kMin + gap;
-                    }
-                    else
-                    {
-                        int32_t penalty = max(kMin, static_cast<int32_t>(prow0[0]));
-                        if (pc == 2)
-                            penalty = max(penalty, static_cast<int32_t>(prow1[0]));
-                        first = penalty + gap;
-                    }
-                }
-                local0 = (bs == 0) ? (pc == 0 ? gap : first) : kMin;
-                carry0 = (pc == 0) ? 0 : first;
-#pragma unroll
-                for (int32_t ci = 0; ci < kMaxChunksPerWarp; ci++)
-                {
-                    const int32_t c = warp + ci * nw_eff;
-                    if (c < nchunks)
-                    {
-                        const int32_t read_pos = bs + c * 128 + 4 * lane;
-                        const uint32_t rd4     = *reinterpret_cast<const uint32_t*>(sread + read_pos);
-                        const int32_t q0       = (base == static_cast<int32_t>(rd4 & 0xff)) ? match : mismatch;
-                        const int32_t q1       = (base == static_cast<int32_t>((rd4 >> 8) & 0xff)) ? match : mismatch;
-                        const int32_t q2       = (base == static_cast<int32_t>((rd4 >> 16) & 0xff)) ? match : mismatch;
-                        const int32_t q3       = (base == static_cast<int32_t>(rd4 >> 24)) ? match : mismatch;
-                        int32_t s0 = kMin, s1 = kMin, s2 = kMin, s3 = kMin;
-                        if (read_pos >= bsp0 && read_pos <= bep0)
-                        {
-                            int32_t b0, b1, b2, b3, b4;
-                            load5<ScoreT>(prow0 + (read_pos - bsp0), b0, b1, b2, b3, b4);
-                            s0 = static_cast<ScoreT>(max(b0 + q0, b1 + gap));
-                            s1 = static_cast<ScoreT>(max(b1 + q1, b2 + gap));
-                            s2 = static_cast<ScoreT>(max(b2 + q2, b3 + gap));
-                            s3 = static_cast<ScoreT>(max(b3 + q3, b4 + gap));
-                        }
-                        if (read_pos >= bsp1 && read_pos <= bep1)
-                        {
-                            int32_t b0, b1, b2, b3, b4;
-                            load5<ScoreT>(prow1 + (read_pos - bsp1), b0, b1, b2, b3, b4);
-                            s0 = max(s0, static_cast<int32_t>(static_cast<ScoreT>(max(b0 + q0, b1 + gap))));
-                            s1 = max(s1, static_cast<int32_t>(static_cast<ScoreT>(max(b1 + q1, b2 + gap))));
-                            s2 = max(s2, static_cast<int32_t>(static_cast<ScoreT>(max(b2 + q2, b3 + gap))));
-                            s3 = max(s3, static_cast<int32_t>(static_cast<ScoreT>(max(b3 + q3, b4 + gap))));
-                        }
-                        closure4(s0, s1, s2, s3, kNegInf, gap, lane);
-                        a0[ci] = s0;
-                        a1[ci] = s1;
-                        a2[ci] = s2;
-                        a3[ci] = s3;
-                        if (lane == 31)
-                            xchg[c] = s3;
-                    }
-                }
-            }
-            else
-            {
-                // ---- general case: any number of predecessors, rows older than the ring come from global memory
-                const int32_t node_id = __shfl_sync(kFull, cur_node, k);
-                const int32_t p0      = __shfl_sync(kFull, cur_p0, k);
-                const int32_t p1      = __shfl_sync(kFull, cur_p1, k);
-                auto pred_row_ptr = [&](int32_t p) -> const ScoreT* {
-                    const int32_t d = row - p;
-                    if (use_ring && d < R)
-                    {
-                        int32_t sl = ring_slot - d;
-                        if (sl < 0)
-                            sl += R;
-                        return ring + sl * stride;
-                    }
-                    return B.row_ptr(p);
-                };
-                int32_t first = 0;
-                if (pc != 0)
-                {
-                    if (bs > kCPT && pc == 1)
-                    {
-                        first = kMin + gap;
-                    }
-                    else
-                    {
-                        int32_t penalty = kMin;
-                        for (int32_t p = 0; p < pc; p++)
-                        {
-                            const int32_t pi = (p == 0) ? p0 : (p == 1 ? p1 : static_cast<int32_t>(g.pos[g.in_edge(node_id, p)]) + 1);
-                            penalty          = max(penalty, static_cast<int32_t>(pred_row_ptr(pi)[0]));
-                        }
-                        first = penalty + gap;
-                    }
-                }
-                local0 = (bs == 0) ? (pc == 0 ? gap : first) : kMin;
-                carry0 = (pc == 0) ? 0 : first;
-                for (int32_t ci = 0; ci < kMaxChunksPerWarp; ci++)
-                {
-                    const int32_t c = warp + ci * nw_eff;
-                    if (c < nchunks)
-                    {
-                        const int32_t read_pos = bs + c * 128 + 4 * lane;
-                        const uint32_t rd4     = *reinterpret_cast<const uint32_t*>(sread + read_pos);
-                        const int32_t q0       = (base == static_cast<int32_t>(rd4 & 0xff)) ? match : mismatch;
-                        const int32_t q1       = (base == static_cast<int32_t>((rd4 >> 8) & 0xff)) ? match : mismatch;
-                        const int32_t q2       = (base == static_cast<int32_t>((rd4 >> 16) & 0xff)) ? match : mismatch;
-                        const int32_t q3       = (base == static_cast<int32_t>(rd4 >> 24)) ? match : mismatch;
-                        int32_t s0 = kMin, s1 = kMin, s2 = kMin, s3 = kMin;
-                        const int32_t np = max(pc, 1);
-                        for (int32_t p = 0; p < np; p++)
-                        {
-                            const int32_t pi  = (p == 0) ? p0 : (p == 1 ? p1 : static_cast<int32_t>(g.pos[g.in_edge(node_id, p)]) + 1);
-                            const int32_t bsp = B.start(pi);
-                            const int32_t bep = min(bsp + band_width - kCPT, max_column);
-                            int32_t t0 = kMin, t1 = kMin, t2 = kMin, t3 = kMin;
-                            if (!(read_pos > bep || read_pos < bsp))
-                            {
-                                int32_t b0, b1, b2, b3, b4;
-                                load5<ScoreT>(pred_row_ptr(pi) + (read_pos - bsp), b0, b1, b2, b3, b4);
-                                t0 = static_cast<ScoreT>(max(b0 + q0, b1 + gap));
-                                t1 = static_cast<ScoreT>(max(b1 + q1, b2 + gap));
-                                t2 = static_cast<ScoreT>(max(b2 + q2, b3 + gap));
-                                t3 = static_cast<ScoreT>(max(b3 + q3, b4 + gap));
-                            }
-                            s0 = (p == 0) ? t0 : max(s0, t0);
-                            s1 = (p == 0) ? t1 : max(s1, t1);
-                            s2 = (p == 0) ? t2 : max(s2, t2);
-                            s3 = (p == 0) ? t3 : max(s3, t3);
-                        }
-                        closure4(s0, s1, s2, s3, kNegInf, gap, lane);
-                        // kMaxChunksPerWarp is small: select the slot without dynamic register indexing
-#pragma unroll
-                        for (int32_t u = 0; u < kMaxChunksPerWarp; u++)
-                        {
-                            if (u == ci)
-                            {
-                                a0[u] = s0;
-                                a1[u] = s1;
-                                a2[u] = s2;
-                                a3[u] = s3;
-                            }
-                        }
-                        if (lane == 31)
-                            xchg[c] = s3;
-                    }
-                }
-            }
-#ifdef GWB200_ROW_PROFILE
-            const unsigned long long rp_t1 = clock64();
-#endif
-            row_sync();
-#ifdef GWB200_ROW_PROFILE
-            const unsigned long long rp_t2 = clock64();
-#endif
-
-            // ---- phase 2: carry into every chunk by a lane-wise max-plus scan over the chunk-out values, final values, stores
-            // lane l < nchunks holds the closed out-value of chunk l rebased to column 0; the carry into chunk c is the maximum
-            // over the chunks to its left (one redux per owned chunk instead of a shuffle scan)
-            const int32_t xv = (lane < nchunks) ? (xchg[lane] - (lane + 1) * G) : kNegInf;
-#pragma unroll
-            for (int32_t ci = 0; ci < kMaxChunksPerWarp; ci++)
-            {
-                const int32_t c = warp + ci * nw_eff;
-                if (c < nchunks)
-                {
-                    const int32_t xm    = __reduce_max_sync(kFull, lane < c ? xv : kNegInf);
-                    const int32_t cin   = static_cast<ScoreT>(c * G + max(carry0, xm)); // closed value of the cell left of chunk c
-                    const int32_t cleft = (c == 0) ? local0 : cin;
-                    const int32_t L     = cin + 4 * gap * lane;
-                    const int32_t s0    = static_cast<ScoreT>(max(a0[ci], L + gap));
-                    const int32_t s1    = static_cast<ScoreT>(max(a1[ci], L + 2 * gap));
-                    const int32_t s2    = static_cast<ScoreT>(max(a2[ci], L + 3 * gap));
-                    const int32_t s3    = static_cast<ScoreT>(max(a3[ci], L + 4 * gap));
-                    int32_t left        = __shfl_up_sync(kFull, s3, 1);
-                    if (lane == 0)
-                        left = cleft;
-                    Vec4<ScoreT> out;
-                    out.x = static_cast<ScoreT>(left);
-                    out.y = static_cast<ScoreT>(s0);
-                    out.z = static_cast<ScoreT>(s1);
-                    out.w = static_cast<ScoreT>(s2);
-                    const int32_t o = c * 128 + 4 * lane;
-                    *reinterpret_cast<Vec4<ScoreT>*>(rowp + o) = out;
-                    if (use_ring)
-                        *reinterpret_cast<Vec4<ScoreT>*>(srow + o) = out;
-                    if (c == nchunks - 1)
-                    {
-                        // last real cell (local band_width) + right padding: lane 31 holds the last cell
-                        if (lane >= 30)
-                        {
-                            Vec4<ScoreT> tl;
-                            tl.x = static_cast<ScoreT>(lane == 31 ? s3 : kMin);
-                            tl.y = static_cast<ScoreT>(kMin);
-                            tl.z = static_cast<ScoreT>(kMin);
-                            tl.w = static_cast<ScoreT>(kMin);
-                            const int32_t to = band_width + 4 * (31 - lane);
-                            *reinterpret_cast<Vec4<ScoreT>*>(rowp + to) = tl;
-                            if (use_ring)
-                                *reinterpret_cast<Vec4<ScoreT>*>(srow + to) = tl;
-                        }
-                    }
-                }
-            }
-#ifdef GWB200_ROW_PROFILE
-            const unsigned long long rp_t3 = clock64();
-#endif
-            row_sync();
-#ifdef GWB200_ROW_PROFILE
-            const unsigned long long rp_t4 = clock64();
-            if (GWB200_ROW_PROFILE == 1)
-            {
-                rp_a += rp_t1 - rp_t0;
-                rp_b += rp_t2 - rp_t1;
-            }
-            else
-            {
-                rp_a += rp_t3 - rp_t2;
-                rp_b += rp_t4 - rp_t3;
-            }
-#endif
-        }
-    }
-#ifdef GWB200_ROW_PROFILE
-    if (timers && threadIdx.x == 0)
-    {
-        timers[6] += rp_a;
-        timers[7] += rp_b;
-    }
-#endif
-    GWB200_TIMER_LAP(0);
-
-    int32_t result = 0;
-    if (warp == 0)
-    {
-    // ---- end cell: first strict maximum over sink rows at column read_length (cudapoa_nw_banded.cuh:407-426)
-    int32_t i = 0;
-    {
-        int32_t best_s = kMin, best_i = 0;
-        for (int32_t idx = 1 + lane; idx <= graph_count; idx += 32)
-        {
-            const int32_t misc = row_meta[idx].w;
-            if ((misc >> 16) & 1)
-            {
-                const int32_t s = B.get(idx, read_length);
-                if (best_s < s)
-                {
-                    best_s = s;
-                    best_i = idx;
-                }
-            }
-        }
-#pragma unroll
-        for (int32_t d = 16; d >= 1; d >>= 1)
-        {
-            const int32_t os = __shfl_xor_sync(kFull, best_s, d);
-            const int32_t oi = __shfl_xor_sync(kFull, best_i, d);
-            if (os > best_s || (os == best_s && oi < best_i))
-            {
-                best_s = os;
-                best_i = oi;
-            }
-        }
-        i = best_i;
-    }
-    GWB200_TIMER_LAP(1);
-
-    // ---- traceback (cudapoa_nw_banded.cuh:428-549): warp-uniform walk over a shared-memory tile
-    ScoreT* tile = reinterpret_cast<ScoreT*>(pool);                                         // [kTileRows][kTileCols]
-    int4* tmeta  = reinterpret_cast<int4*>(pool + kTileRows * kTileCols * sizeof(ScoreT)); // [kTileRows]
-    uint8_t* tread = reinterpret_cast<uint8_t*>(tmeta + kTileRows);                          // read[J0 - 1 + k], k in [0, 66)
-    int8_t* tjump  = reinterpret_cast<int8_t*>(tread + 72);                                  // [5][kTileRows]: 2^m-th pred0 ancestor
-    int32_t t_lo = 1, t_hi = 0, J0 = 0; // tile rows [t_lo, t_hi], columns [J0, J0 + kTileCols)
-
-    auto refill = [&](int32_t ri, int32_t rj) {
-        __syncwarp();
-        t_hi = ri;
-        t_lo = max(0, ri - (kTileRows - 1));
-        J0   = max(0, rj - (kTileCols - 2)) & ~1;
-        {
-            const int32_t row = t_lo + lane; // metadata: lane k <-> row t_lo + k
-            int32_t up        = -1;          // tile-relative row of the first predecessor, -1 = none inside the tile
-            if (row <= t_hi)
-            {
-                const int4 mm = row >= 1 ? row_meta[row] : make_int4(0, 0, 0, 0);
-                tmeta[lane]   = mm;
-                if (row >= 1 && mm.y >= t_lo)
-                    up = mm.y - t_lo;
-            }
-            // pointer doubling over the first-predecessor links: tjump[m][r] = 2^m-th ancestor of tile row r (or -1)
-            tjump[lane] = static_cast<int8_t>(up);
-#pragma unroll
-            for (int32_t m = 1; m < 5; m++)
-            {
-                __syncwarp();
-                if (up >= 0)
-                    up = tjump[(m - 1) * kTileRows + up];
-                tjump[m * kTileRows + lane] = static_cast<int8_t>(up);
-            }
-        }
-        for (int32_t k = lane; k < kTileCols + 2; k += 32)
-        {
-            const int32_t rp = J0 - 1 + k;
-            tread[k]         = (rp >= 0 && rp < read_length) ? __ldg(read + rp) : 0;
-        }
-        // scores: one row per iteration, 2 columns per lane, band test as get_score() does (:80-102)
-        const int32_t nr = t_hi - t_lo;
-#pragma unroll 8
-        for (int32_t r = 0; r <= nr; r++)
-        {
-            const int32_t row = t_lo + r;
-            const int32_t bs  = B.start(row);
-            const int32_t be  = min(bs + band_width, max_column);
-            const int32_t J   = J0 + 2 * lane;
-            int32_t v0 = kMin, v1 = kMin;
-            const ScoreT* rp = B.row_ptr(row);
-            if (J >= bs && J <= be)
-                v0 = rp[J - bs];
-            if (J + 1 >= bs && J + 1 <= be)
-                v1 = rp[J + 1 - bs];
-            tile[r * kTileCols + 2 * lane]     = static_cast<ScoreT>(v0);
-            tile[r * kTileCols + 2 * lane + 1] = static_cast<ScoreT>(v1);
-        }
-        __syncwarp();
-    };
-    // score as the reference's get_score(row, column) sees it: tile hit, else the (rare) global-memory path
-    auto T = [&](int32_t row, int32_t column) -> int32_t {
-        const uint32_t r = static_cast<uint32_t>(row - t_lo);
-        const uint32_t c = static_cast<uint32_t>(column - J0);
-        if (r <= static_cast<uint32_t>(t_hi - t_lo) && c < static_cast<uint32_t>(kTileCols))
-            return tile[r * kTileCols + c];
-        return band_get_slow<ScoreT>(B, row, column);
-    };
-
-    int32_t aligned_nodes = 0;
-    {
-        int32_t j      = read_length;
-        int32_t prev_i = 0, prev_j = 0;
-        int32_t next_node_id    = i > 0 ? row_meta[i].x : 0;
-        int32_t loop_count      = 0;
-        const int32_t limit     = read_length + graph_count + 2;
-        const int32_t threshold = max(1, max_column / 1024);
-        const bool check_band   = Adaptive && rerun == 0 && band_width < kMaxAdaptiveBW;
-        while (!(i == 0 && j == 0) && loop_count < limit)
-        {
-            loop_count++;
-            if (i < t_lo || i > t_hi || j >= J0 + kTileCols || (j > 0 && j - 1 < J0))
-                refill(i, j);
-            // ---- speculative run: lane k assumes the previous k steps were all "diagonal through the first predecessor" (the
-            // first test of every step, :467-478), finds the row it would stand on by following k first-predecessor links
-            // (binary decomposition of k over the tile's pointer-doubling tables) and verifies its own step on the tile; the
-            // leading run of successful lanes is exactly what the serial loop would do for those steps, taken at once.
-            {
-                int32_t pos = i - t_lo; // tile-relative row after `lane` steps, -1 = outside the tile
-#pragma unroll
-                for (int32_t m = 0; m < 5; m++)
-                {
-                    if (((lane >> m) & 1) && pos >= 0)
-                        pos = tjump[m * kTileRows + pos];
-                }
-                const int32_t ik = t_lo + pos;
-                const int32_t jk = j - lane;
-                bool ok          = pos >= 0 && ik >= 1 && jk >= 1 && (jk - 1) >= J0 && (loop_count - 1 + lane) < limit;
-                int32_t knode = 0, kup = 0;
-                if (ok)
-                {
-                    const int4 mk = tmeta[pos];
-                    knode         = mk.x;
-                    kup           = mk.y; // first predecessor row (row 0 for source nodes)
-                    ok            = kup >= t_lo;
-                    if (check_band && jk > threshold && jk < max_column - threshold)
-                    {
-                        const int32_t bsk = ((mk.w >> 17) & 0x3fff) << 2;
-                        if (jk <= bsk + threshold || jk >= (bsk + band_width - threshold))
-                            ok = false; // the serial step below performs the abort
-                    }
-                    if (ok)
-                    {
-                        const int32_t cost = ((mk.w & 0xff) == static_cast<int32_t>(tread[jk - J0])) ? match : mismatch;
-                        const int32_t sij  = tile[pos * kTileCols + (jk - J0)];
-                        const int32_t sd   = tile[(kup - t_lo) * kTileCols + (jk - 1 - J0)];
-                        ok                 = sij == sd + cost;
-                    }
-                }
-                // the first step uses next_node_id, which must be the node of row i for the speculation to be the serial behaviour
-                const int32_t node0 = __shfl_sync(kFull, knode, 0);
-                uint32_t okmask     = __ballot_sync(kFull, ok);
-                if (node0 != next_node_id)
-                    okmask = 0u;
-                const int32_t run = (okmask == kFull) ? 32 : (__ffs(~okmask) - 1);
-                if (run > 0)
-                {
-                    if (lane < run)
-                    {
-                        aln_graph[aligned_nodes + lane] = static_cast<SizeT>(knode);
-                        aln_read[aligned_nodes + lane]  = static_cast<SizeT>(jk - 1);
-                    }
-                    aligned_nodes += run;
-                    loop_count += run - 1; // the loop header already counted one step
-                    i = __shfl_sync(kFull, kup, run - 1);
-                    j -= run;
-                    prev_i = i;
-                    prev_j = j;
-                    if (i > 0)
-                    {
-                        const uint32_t r = static_cast<uint32_t>(i - t_lo);
-                        next_node_id     = (r <= static_cast<uint32_t>(t_hi - t_lo)) ? tmeta[r].x : row_meta[i].x;
-                    }
-                    else
-                    {
-                        next_node_id = 0;
-                    }
-                    continue;
-                }
-            }
-            const int32_t ti        = i - t_lo;
-            const int32_t tj        = j - J0;
-            const int32_t scores_ij = tile[ti * kTileCols + tj];
-            const int4 m            = tmeta[ti];
-            const int32_t row_node  = m.x; // graph[i - 1]
-            const int32_t pc_i      = (m.w >> 8) & 0xff;
-            bool pred_found         = false;
-            if (i != 0 && j != 0)
-            {
-                if (check_band && j > threshold && j < max_column - threshold)
-                {
-                    const int32_t bs = ((m.w >> 17) & 0x3fff) << 2; // band start of row i, packed by the DP phase
-                    if (j <= bs + threshold)
-                    {
-                        aligned_nodes = kShiftLeft;
-                        break;
-                    }
-                    if (j >= (bs + band_width - threshold))
-                    {
-                        aligned_nodes = kShiftRight;
-                        break;
-                    }
-                }
-                // the reference uses next_node_id (= graph[prev_i - 1] of the previous step) here; it equals graph[i - 1]
-                // whenever the previous step found a predecessor and is stale otherwise -- that behaviour is kept
-                const int32_t node_id = next_node_id;
-                int32_t nbase = m.w & 0xff, pc = pc_i, pred_i = m.y;
-                if (node_id != row_node)
-                {
-                    nbase  = g.nodes[node_id];
-                    pc     = g.in_cnt[node_id];
-                    pred_i = (pc == 0) ? 0 : (static_cast<int32_t>(g.pos[g.in_edge(node_id, 0)]) + 1);
-                }
-                const int32_t match_cost = (nbase == static_cast<int32_t>(tread[tj])) ? match : mismatch; // read[j - 1]
-                if (scores_ij == (T(pred_i, j - 1) + match_cost))
-                {
-                    prev_i     = pred_i;
-                    prev_j     = j - 1;
-                    pred_found = true;
-                }
-                else
-                {
-                    for (int32_t p = 1; p < pc; p++)
-                    {
-                        pred_i = (p == 1 && node_id == row_node) ? m.z : (static_cast<int32_t>(g.pos[g.in_edge(node_id, p)]) + 1);
-                        if (scores_ij == (T(pred_i, j - 1) + match_cost))
-                        {
-                            prev_i     = pred_i;
-                            prev_j     = j - 1;
-                            pred_found = true;
-                            break;
-                        }
-                    }
-                }
-            }
-            if (!pred_found && i != 0)
-            {
-                int32_t pred_i = (pc_i == 0) ? 0 : m.y;
-                if (scores_ij == T(pred_i, j) + gap)
-                {
-                    prev_i     = pred_i;
-                    prev_j     = j;
-                    pred_found = true;
-                }
-                else
-                {
-                    for (int32_t p = 1; p < pc_i; p++)
-                    {
-                        pred_i = (p == 1) ? m.z : (static_cast<int32_t>(g.pos[g.in_edge(row_node, p)]) + 1);
-                        if (scores_ij == T(pred_i, j) + gap)
-                        {
-                            prev_i     = pred_i;
-                            prev_j     = j;
-                            pred_found = true;
-                            break;
-                        }
-                    }
-                }
-            }
-            if (!pred_found && scores_ij == T(i, j - 1) + gap)
-            {
-                prev_i     = i;
-                prev_j     = j - 1;
-                pred_found = true;
-            }
-            // next_node_id = graph[prev_i - 1]
-            if (prev_i > 0)
-            {
-                const uint32_t r = static_cast<uint32_t>(prev_i - t_lo);
-                next_node_id     = (r <= static_cast<uint32_t>(t_hi - t_lo)) ? tmeta[r].x : row_meta[prev_i].x;
-            }
-            else
-            {
-                next_node_id = 0;
-            }
-            if (lane == 0)
-            {
-                aln_graph[aligned_nodes] = static_cast<SizeT>((i == prev_i) ? -1 : row_node);
-                aln_read[aligned_nodes]  = static_cast<SizeT>((j == prev_j) ? -1 : j - 1);
-            }
-            aligned_nodes++;
-            i = prev_i;
-            j = prev_j;
-        }
-        if (loop_count >= limit)
-            aligned_nodes = kNWBacktrackFail;
-    }
-    __syncwarp();
-    result = aligned_nodes;
-    if (lane == 0)
-        s_xchg[32] = result;
-    } // warp 0
-    __syncthreads();
-    result = s_xchg[32];
-    __syncthreads();
-    GWB200_TIMER_LAP(2);
-    return result;
 }
 
 // addAlignmentToGraph (cudapoa_add_alignment.cuh:65-285), lane-parallel over read bases. rd_node[r] = graph node aligned
@@ -1133,256 +374,6 @@ __device__ void topsort_v2(const Win<SizeT>& g, int32_t node_count, uint8_t* poo
         if ((threadIdx.x & 31) == 0)
             topsort(g, node_count);
         __syncwarp();
-    }
-}
-
-template <typename ScoreT, typename SizeT, int32_t NW, int32_t MAXC>
-__global__ void __launch_bounds__(32 * NW, (NW == 4 ? GWB200_POA_NW4_BLOCKS : (NW == 1 ? 16 : 10))) poa_window_kernel_v2(const DeviceParams P, const V2Extra X)
-{
-    const bool MSA = P.msa != 0;
-    extern __shared__ __align__(16) uint8_t pool[];
-    __shared__ int32_t s_xchg[40]; // [0,32): chunk carry exchange (2 x 16), [32,40): broadcasts from warp 0
-    const int32_t w    = blockIdx.x;
-    const int32_t lane = threadIdx.x & 31;
-    const int32_t warp = threadIdx.x >> 5;
-    if (w >= P.n_windows)
-        return;
-    const WindowInfo wi = P.windows[w];
-    const int64_t mn    = P.max_nodes;
-    unsigned long long* timers = X.timers ? X.timers + static_cast<int64_t>(w) * 8 : nullptr;
-
-    Win<SizeT> g;
-    g.max_nodes = P.max_nodes;
-    g.nodes     = P.nodes + w * mn;
-    g.in_cnt    = P.in_cnt + w * mn;
-    g.out_cnt   = P.out_cnt + w * mn;
-    g.aln_cnt   = P.aln_cnt + w * mn;
-    g.cov       = P.node_cov + w * mn;
-    g.local_cnt = P.local_cnt + w * mn;
-    g.in_edges  = static_cast<SizeT*>(P.in_edges) + w * mn * kMaxEdges;
-    g.out_edges = static_cast<SizeT*>(P.out_edges) + w * mn * kMaxEdges;
-    g.aligned   = static_cast<SizeT*>(P.aligned) + w * mn * kMaxAligned;
-    g.in_w      = P.in_w + w * mn * kMaxEdges;
-    g.sorted    = static_cast<SizeT*>(P.sorted) + w * mn;
-    g.pos       = static_cast<SizeT*>(P.pos) + w * mn;
-
-    SizeT* aln_graph = static_cast<SizeT*>(P.aln_graph) + static_cast<int64_t>(w) * P.aln_capacity;
-    SizeT* aln_read  = static_cast<SizeT*>(P.aln_read) + static_cast<int64_t>(w) * P.aln_capacity;
-    int4* row_meta   = X.row_meta + static_cast<int64_t>(w) * (mn + 1);
-    SizeT* rd_node   = static_cast<SizeT*>(X.rd_node) + static_cast<int64_t>(w) * X.rd_capacity;
-
-    const int32_t* seq_lengths = P.seq_lengths + wi.seq_len_offset;
-    const uint8_t* sequence    = P.sequences + wi.seq_start;
-    const int8_t* base_weights = P.weights + wi.seq_start;
-    SizeT* path                = MSA ? static_cast<SizeT*>(P.seq_path) + wi.seq_start : nullptr;
-
-    float banded_buffer_size = static_cast<float>(P.max_nodes) * static_cast<float>(P.matrix_seq_dim);
-    ScoreT* scores;
-    if (P.band_mode == bm_full_band)
-        scores = static_cast<ScoreT*>(P.scores) + wi.scores_offset * mn;
-    else
-        scores = static_cast<ScoreT*>(P.scores) + static_cast<int64_t>(banded_buffer_size) * static_cast<int64_t>(w);
-
-    uint8_t* consensus = P.consensus + static_cast<int64_t>(w) * P.max_consensus;
-    uint16_t* coverage = P.coverage + static_cast<int64_t>(w) * P.max_consensus;
-
-    // a group whose reads were all rejected stays in the batch with no read (add_poa_group returns empty_poa_group,
-    // cudapoa_batch.cuh:139-148): nothing to align, and seq_lengths[0] would belong to another window
-    if (wi.num_seqs <= 0)
-    {
-        if (threadIdx.x == 0)
-        {
-            consensus[0]       = 0;
-            P.status[w]        = st_empty_poa_group;
-            P.consensus_len[w] = 0;
-            P.node_count[w]    = 0;
-            P.cells[w]         = 0;
-        }
-        return;
-    }
-    // backbone from read 0 (cudapoa_kernels.cuh:200-238), thread-parallel
-    int32_t node_count = seq_lengths[0];
-    for (int32_t n = threadIdx.x; n < node_count; n += 32 * NW)
-    {
-        g.nodes[n]   = sequence[n];
-        g.sorted[n]  = static_cast<SizeT>(n);
-        g.pos[n]     = static_cast<SizeT>(n);
-        g.aln_cnt[n] = 0;
-        g.cov[n]     = 1;
-        if (n > 0)
-        {
-            g.in_edge(n, 0)      = static_cast<SizeT>(n - 1);
-            g.w(n, 0)            = static_cast<uint16_t>(base_weights[n - 1] + base_weights[n]);
-            g.in_cnt[n]          = 1;
-            g.out_edge(n - 1, 0) = static_cast<SizeT>(n);
-            g.out_cnt[n - 1]     = 1;
-        }
-        else
-        {
-            g.in_cnt[0] = 0;
-            g.w(0, 0)   = static_cast<uint16_t>(base_weights[0]);
-        }
-        if (n == node_count - 1)
-            g.out_cnt[n] = 0;
-        if (MSA)
-            path[n] = static_cast<SizeT>(n);
-    }
-    __syncthreads();
-
-    unsigned long long cells = 0;
-    int32_t error            = 0;
-    const int32_t num_seqs   = wi.num_seqs;
-
-    for (int32_t s = 1; s < num_seqs; s++)
-    {
-        const int32_t seq_len = seq_lengths[s];
-        const int32_t adv     = (seq_lengths[s - 1] + 3) & ~3;
-        sequence += adv;
-        base_weights += adv;
-        if (MSA)
-            path += adv;
-        if (node_count >= P.max_nodes)
-        {
-            error = st_node_count_exceeded_maximum_graph_size;
-            break;
-        }
-        int32_t alen;
-        if (P.band_mode == bm_static_band_traceback || P.band_mode == bm_adaptive_band_traceback)
-        {
-            // cudapoa_kernels.cuh:270-346; served by the one-warp kernel only (the host selects it)
-            alen = kNWBacktrackFail;
-            if constexpr (NW == 1 && MAXC == 1)
-            {
-                const bool adaptive = (P.band_mode == bm_adaptive_band_traceback && P.band_width < kMaxAdaptiveBW);
-                ScoreT* tb_scores   = static_cast<ScoreT*>(X.tb_scores) + static_cast<int64_t>(w) * X.tb_height * P.matrix_seq_dim;
-                const int64_t toff  = static_cast<int64_t>(banded_buffer_size) * static_cast<int64_t>(w);
-                int32_t rerun       = 0;
-                for (int32_t attempt = 0; attempt < 2; attempt++)
-                {
-                    if (X.tb_trace16)
-                        alen = nw_banded_tb<ScoreT, SizeT, int16_t>(g, node_count, sequence, seq_len, tb_scores, static_cast<int16_t*>(X.tb_trace) + toff,
-                                                                    banded_buffer_size, aln_graph, aln_read, P.band_width, X.tb_height, P.gap,
-                                                                    P.mismatch, P.match, rerun, adaptive, cells);
-                    else
-                        alen = nw_banded_tb<ScoreT, SizeT, int8_t>(g, node_count, sequence, seq_len, tb_scores, static_cast<int8_t*>(X.tb_trace) + toff,
-                                                                   banded_buffer_size, aln_graph, aln_read, P.band_width, X.tb_height, P.gap,
-                                                                   P.mismatch, P.match, rerun, adaptive, cells);
-                    if (!adaptive || attempt == 1 || !(alen == kShiftLeft || alen == kShiftRight))
-                        break;
-                    rerun = alen;
-                }
-            }
-            if (alen == kNWTracebackBufferFail)
-            {
-                error = st_exceeded_maximum_predecessor_distance;
-                break;
-            }
-        }
-        else if (P.band_mode != bm_full_band)
-        {
-            const bool adaptive = (P.band_mode == bm_adaptive_band && P.band_width < kMaxAdaptiveBW);
-            int32_t rerun       = 0;
-            for (int32_t attempt = 0; attempt < 2; attempt++)
-            {
-                alen = nw_banded_v2<ScoreT, SizeT, NW, MAXC>(g, node_count, sequence, seq_len, scores, banded_buffer_size, aln_graph, aln_read,
-                                                            P.band_width, P.gap, P.mismatch, P.match, rerun, adaptive, cells, row_meta, pool,
-                                                            X.pool_bytes, timers, s_xchg);
-                if (!adaptive || attempt == 1 || !(alen == kShiftLeft || alen == kShiftRight))
-                    break;
-                rerun = alen; // rerun with extended and shifted band (cudapoa_kernels.cuh:374-396)
-            }
-        }
-        else
-        {
-            if (warp == 0)
-            {
-                alen = nw_full<ScoreT, SizeT>(g, node_count, sequence, seq_len, scores, wi.scores_width, aln_graph, aln_read, P.gap,
-                                              P.mismatch, P.match, cells);
-                if (lane == 0)
-                    s_xchg[32] = alen;
-            }
-            __syncthreads();
-            alen = s_xchg[32];
-            __syncthreads();
-        }
-        if (alen == kNWBacktrackFail)
-        {
-            error = st_loop_count_exceeded_upper_bound;
-            break;
-        }
-        if (alen == kNWStorageFail)
-        {
-            error = st_exceeded_adaptive_banded_matrix_size;
-            break;
-        }
-        if (alen < 0)
-            alen = 0;
-        {
-            unsigned long long t_ph__ = timers ? clock64() : 0ull;
-            if (warp == 0)
-            {
-                int32_t nc = node_count;
-                int32_t e  = add_alignment_v2<SizeT>(g, nc, alen, aln_graph, sequence, seq_len, aln_read, base_weights, path, rd_node);
-                GWB200_TIMER_LAP(3);
-                if (!e)
-                {
-                    if (P.accurate)
-                    {
-                        if ((threadIdx.x & 31) == 0)
-                            racon_topsort(g, nc, P.marks + w * mn, P.check + w * mn,
-                                          static_cast<SizeT*>(P.stack) + static_cast<int64_t>(w) * P.stack_capacity, P.stack_capacity);
-                        __syncwarp();
-                    }
-                    else
-                    {
-                        topsort_v2<SizeT>(g, nc, pool, X.pool_bytes, static_cast<SizeT*>(P.cons_preds) + w * mn);
-                    }
-                }
-                GWB200_TIMER_LAP(4);
-                if (lane == 0)
-                {
-                    s_xchg[33] = e;
-                    s_xchg[34] = nc;
-                }
-            }
-            __syncthreads();
-            error      = s_xchg[33];
-            node_count = s_xchg[34];
-            __syncthreads();
-            if (error)
-                break;
-        }
-    }
-
-    int32_t cons_len = 0;
-    if (!error && warp == 0)
-    {
-        unsigned long long t_ph__ = timers ? clock64() : 0ull;
-        if (MSA)
-        {
-            error = generate_msa<SizeT>(g, node_count, num_seqs, seq_lengths, static_cast<SizeT*>(P.seq_path) + wi.seq_start,
-                                        static_cast<SizeT*>(P.msa_col) + w * mn, P.marks + w * mn, P.check + w * mn,
-                                        static_cast<SizeT*>(P.stack) + static_cast<int64_t>(w) * P.stack_capacity, P.stack_capacity,
-                                        P.msa_out + static_cast<int64_t>(w) * P.max_seqs * P.max_consensus, P.max_consensus);
-        }
-        else
-        {
-            error = generate_consensus<SizeT>(g, node_count, P.cons_scores + w * mn, static_cast<SizeT*>(P.cons_preds) + w * mn, consensus,
-                                              coverage, P.max_consensus, &cons_len);
-        }
-        GWB200_TIMER_LAP(5);
-    }
-    if (threadIdx.x == 0)
-    {
-        if (error)
-        {
-            consensus[0] = 0;
-            cons_len     = 0;
-        }
-        P.status[w]        = error;
-        P.consensus_len[w] = cons_len;
-        P.node_count[w]    = node_count;
-        P.cells[w]         = cells;
     }
 }
 

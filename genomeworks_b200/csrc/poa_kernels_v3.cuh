@@ -1,8 +1,7 @@
 // gw-b200 POA device code, third generation (sm_90a): one warp per window, persistent CTAs, 8 score cells per lane and chunk.
 //
-// Same behavioural contract as poa_kernels.cuh / poa_kernels_v2.cuh (identical consensus / coverage / MSA / status to the
-// reference kernels, cudapoa/src/cudapoa_kernels.cuh:76-542). What changed against v2, and why (v2 parks three
-// of four warps at CTA barriers through traceback / graph update / sort and at every row barrier):
+// Same behavioural contract as poa_kernels.cuh (identical consensus / coverage / MSA / status to the reference kernels,
+// cudapoa/src/cudapoa_kernels.cuh:76-542). The graph update is add_alignment_v2 (poa_kernels_v2.cuh).
 //
 //   scheduling   one warp owns one window from the first read to the consensus; the grid is persistent (resident CTAs pull
 //                window indices from an atomic counter), so every resident warp always has work of its own, no CTA barrier
@@ -20,7 +19,9 @@
 //                stores in the row loop, and the ring slot is reused only after its bulk read has completed.
 //   traceback    score tiles (32 rows x 64 columns), the rows' metadata and the next tile along the predicted path are
 //                fetched by bulk asynchronous copies that complete on an mbarrier (cp.async.bulk.shared::cluster.global);
-//                the walk itself is v2's speculative warp-uniform walk (reference order cudapoa_nw_banded.cuh:440-534).
+//                the walk is warp-uniform and keeps the reference's per-step preference order (cudapoa_nw_banded.cuh:440-534);
+//                runs of "diagonal through the first predecessor" are taken 32 steps at a time (pointer doubling over the
+//                tile's first-predecessor links, lane k verifies step k).
 #pragma once
 #include <type_traits>
 
@@ -84,11 +85,10 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t pari
 struct V3Extra
 {
     int32_t* work_counter; // next window index (persistent grid), reset by the host before every launch
-    int32_t use_bulk;      // 1: rows leave the ring by cp.async.bulk (default); 0: per-lane vector stores (A/B switch)
-    int32_t tb_tma;        // 1: traceback tiles by bulk asynchronous copies with prefetch (default); 0: lane loads (A/B switch)
-    int32_t wavefront;     // 1: 32-bit score rows as a skewed wavefront (poa_kernels_v4.cuh); 0: dp_rows_v3 (default)
-    int32_t max_group;     // chunks per straight-line group of the row loop: 4, 2 or 1 (see dp_rows_v3)
-    int32_t row_fence;     // 1: fence.proxy.async in front of every general row that reads rows older than the ring (A/B switch)
+    // chunks per straight-line group of a fast row with 32-bit scores: 1 (8 cells per lane in flight; 16-bit rows always take
+    // groups of 2). A kernel argument rather than a constant: with the 2-chunk groups compiled out, ptxas lays out the 32-bit
+    // kernel differently and C3 of bench.py measured 5 % slower on an H100
+    int32_t max_group32;
 };
 
 // Static shared memory of the v3 kernel that is not part of the pool
@@ -100,27 +100,13 @@ struct V3Shared
     uint32_t pad_[2];
 };
 
-// 1: a chunk whose entering horizontal run dominates all of its cells is decided by one ballot instead of the prefix scan.
-// Left off: the scan runs in ~57 % of the chunks of a wide band (right of the alignment path every cell is its left neighbour +
-// gap), and the extra ballot sits on the carry chain of every chunk.
-#ifndef GWB200_V3_PURE
-#define GWB200_V3_PURE 0
-#endif
-#ifndef GWB200_V3_CPL32
-#define GWB200_V3_CPL32 8 // 4: one 16-byte unit per lane and chunk (the round-2 layout, kept as the A/B partner)
-#endif
+// cells per lane and chunk: 8 (int16: one 16-byte unit, int32: two), so that the per-chunk costs -- neighbour shuffle, carry
+// shuffles and ballot, addressing, band tests -- are paid once per 256 columns
+constexpr int32_t kCPL   = 8;
+constexpr int32_t kChunk = 32 * kCPL; // columns per chunk
 
+// the kCPL cells of a lane <-> int32 values
 template <typename ScoreT>
-struct V3Cells
-{
-    // cells per lane and chunk: 8 (int16: one 16-byte unit, int32: two), so that the per-chunk costs -- neighbour shuffle, carry
-    // shuffles and ballot, addressing, band tests -- are paid once per 256 columns
-    static constexpr int32_t kCPL   = sizeof(ScoreT) == 2 ? 8 : GWB200_V3_CPL32;
-    static constexpr int32_t kChunk = 32 * kCPL; // columns per chunk
-};
-
-// 16-byte unit <-> CPL int32 values
-template <typename ScoreT, int32_t CPL>
 __device__ __forceinline__ void unit_load(const ScoreT* p, int32_t* b)
 {
     if constexpr (sizeof(ScoreT) == 4)
@@ -130,14 +116,11 @@ __device__ __forceinline__ void unit_load(const ScoreT* p, int32_t* b)
         b[1]         = v.y;
         b[2]         = v.z;
         b[3]         = v.w;
-        if constexpr (CPL == 8)
-        {
-            const int4 u = *reinterpret_cast<const int4*>(p + 4);
-            b[4]         = u.x;
-            b[5]         = u.y;
-            b[6]         = u.z;
-            b[7]         = u.w;
-        }
+        const int4 u = *reinterpret_cast<const int4*>(p + 4);
+        b[4]         = u.x;
+        b[5]         = u.y;
+        b[6]         = u.z;
+        b[7]         = u.w;
     }
     else
     {
@@ -155,15 +138,14 @@ __device__ __forceinline__ void unit_load(const ScoreT* p, int32_t* b)
     }
 }
 
-// unit = {left, s[0], ..., s[CPL-2]} (values already truncated to ScoreT range), 16-byte aligned destination
-template <typename ScoreT, int32_t CPL>
-__device__ __forceinline__ void unit_store(ScoreT* p, int32_t left, const int32_t (&s)[CPL])
+// unit = {left, s[0], ..., s[kCPL-2]} (values already truncated to ScoreT range), 16-byte aligned destination
+template <typename ScoreT>
+__device__ __forceinline__ void unit_store(ScoreT* p, int32_t left, const int32_t (&s)[kCPL])
 {
     if constexpr (sizeof(ScoreT) == 4)
     {
-        *reinterpret_cast<int4*>(p) = make_int4(left, s[0], s[1], s[2]);
-        if constexpr (CPL == 8)
-            *reinterpret_cast<int4*>(p + 4) = make_int4(s[3], s[4], s[5], s[6]);
+        *reinterpret_cast<int4*>(p)     = make_int4(left, s[0], s[1], s[2]);
+        *reinterpret_cast<int4*>(p + 4) = make_int4(s[3], s[4], s[5], s[6]);
     }
     else
     {
@@ -176,23 +158,22 @@ __device__ __forceinline__ void unit_store(ScoreT* p, int32_t left, const int32_
     }
 }
 
-// Closure of s[c] = max(h[c], s[c-1] + gap) over one chunk (CPL consecutive cells per lane) with carry-in `cin` for lane 0:
+// Closure of s[c] = max(h[c], s[c-1] + gap) over one chunk (kCPL consecutive cells per lane) with carry-in `cin` for lane 0:
 // the fixpoint of the reference's relaxation loop (cudapoa_nw_banded.cuh:362-390). `left` returns the closed value of the cell
 // left of this lane's first cell (lane 0: cin). Fast exit when no lane's first cell is improved by its left neighbour.
-template <int32_t CPL>
-__device__ __forceinline__ void closure_seq(int32_t (&s)[CPL], int32_t cin, int32_t gap, int32_t lane, int32_t& left)
+__device__ __forceinline__ void closure_seq(int32_t (&s)[kCPL], int32_t cin, int32_t gap, int32_t lane, int32_t& left)
 {
 #pragma unroll
-    for (int32_t k = 1; k < CPL; k++)
+    for (int32_t k = 1; k < kCPL; k++)
         s[k] = __viaddmax_s32(s[k - 1], gap, s[k]);
-    int32_t nb = __shfl_up_sync(kFull, s[CPL - 1], 1);
+    int32_t nb = __shfl_up_sync(kFull, s[kCPL - 1], 1);
     if (lane == 0)
         nb = cin;
     left = nb;
     if (__ballot_sync(kFull, nb + gap > s[0]) == 0u)
         return;
-    const int32_t gl = CPL * gap;
-    int32_t v        = s[CPL - 1] - gl * (lane + 1);
+    const int32_t gl = kCPL * gap;
+    int32_t v        = s[kCPL - 1] - gl * (lane + 1);
 #pragma unroll
     for (int32_t d = 1; d < 32; d <<= 1)
     {
@@ -204,17 +185,16 @@ __device__ __forceinline__ void closure_seq(int32_t (&s)[CPL], int32_t cin, int3
     excl         = (lane == 0) ? cin : max(cin, excl);
     const int32_t L = excl + gl * lane;
 #pragma unroll
-    for (int32_t k = 0; k < CPL; k++)
+    for (int32_t k = 0; k < kCPL; k++)
         s[k] = max(s[k], L + (k + 1) * gap);
     left = L;
 }
 
 // The max-plus prefix scan of one chunk (the grouped row code below needs it for a minority of its chunks)
-template <int32_t CPL>
-__device__ __forceinline__ int32_t chunk_scan(int32_t (&a)[CPL], const int32_t cin, const int32_t gap, const int32_t lane)
+__device__ __forceinline__ int32_t chunk_scan(int32_t (&a)[kCPL], const int32_t cin, const int32_t gap, const int32_t lane)
 {
-    const int32_t gl = CPL * gap;
-    int32_t v        = a[CPL - 1] - gl * (lane + 1);
+    const int32_t gl = kCPL * gap;
+    int32_t v        = a[kCPL - 1] - gl * (lane + 1);
 #pragma unroll
     for (int32_t d = 1; d < 32; d <<= 1)
     {
@@ -226,7 +206,7 @@ __device__ __forceinline__ int32_t chunk_scan(int32_t (&a)[CPL], const int32_t c
     excl            = (lane == 0) ? cin : max(cin, excl);
     const int32_t L = excl + gl * lane;
 #pragma unroll
-    for (int32_t i = 0; i < CPL; i++)
+    for (int32_t i = 0; i < kCPL; i++)
         a[i] = max(a[i], L + (i + 1) * gap);
     return L;
 }
@@ -238,8 +218,7 @@ struct RowCtx
     const ScoreT* prow0; // ring rows of the predecessors
     const ScoreT* prow1;
     const uint8_t* rd;   // read + band start of the row
-    ScoreT* drow;        // where the lanes write the row (ring slot, or the row in global memory without a ring)
-    ScoreT* grow;        // second copy in global memory (lane stores instead of the bulk copy), or nullptr
+    ScoreT* drow;        // the row's ring slot
     int32_t sh0, lim0, sh1, lim1;
     int32_t base, bw, gap, match, mismatch;
     uint32_t base4; // the row's base in every byte
@@ -252,67 +231,65 @@ template <typename ScoreT, int32_t NJ, bool TWO>
 __device__ __forceinline__ void row_group_v3(const RowCtx<ScoreT>& cx, const int32_t c0, const int32_t lane, int32_t& cin, int32_t& cleft)
 {
     constexpr int32_t kMin = min_score_of<ScoreT>();
-    constexpr int32_t CPL  = V3Cells<ScoreT>::kCPL;
-    constexpr int32_t CH   = V3Cells<ScoreT>::kChunk;
     const int32_t gap      = cx.gap;
-    int32_t a[NJ][CPL];
+    int32_t a[NJ][kCPL];
     int32_t nbraw[NJ], outv[NJ], s0l0[NJ], leftv[NJ];
     uint32_t need[NJ];
     bool act[NJ];
     {
         // ---- loads: read characters and the predecessors' units of every chunk
-        uint32_t w[NJ][CPL / 4];
-        int32_t b0[NJ][CPL + 1], b1[TWO ? NJ : 1][CPL + 1];
+        uint32_t w[NJ][kCPL / 4];
+        int32_t b0[NJ][kCPL + 1], b1[TWO ? NJ : 1][kCPL + 1];
         bool in0[NJ], in1[TWO ? NJ : 1];
 #pragma unroll
         for (int32_t j = 0; j < NJ; j++)
         {
-            const int32_t off = (c0 + j) * CH + CPL * lane;
+            const int32_t off = (c0 + j) * kChunk + kCPL * lane;
             act[j]            = off < cx.bw;
 #pragma unroll
-            for (int32_t h = 0; h < CPL / 4; h++)
+            for (int32_t h = 0; h < kCPL / 4; h++)
                 w[j][h] = __ldg(reinterpret_cast<const uint32_t*>(cx.rd + off + 4 * h)) ^ cx.base4;
             const int32_t o = cx.sh0 + off;
             in0[j]          = act[j] && o <= cx.lim0;
             // lanes outside the predecessor's band load its first unit instead: their values are discarded by ok0 below
-            unit_load<ScoreT, CPL>(cx.prow0 + (in0[j] ? o : 0), b0[j]);
+            unit_load<ScoreT>(cx.prow0 + (in0[j] ? o : 0), b0[j]);
             if (TWO)
             {
                 const int32_t o1 = cx.sh1 + off;
                 in1[j]           = act[j] && o1 <= cx.lim1;
-                unit_load<ScoreT, CPL>(cx.prow1 + (in1[j] ? o1 : 0), b1[j]);
+                unit_load<ScoreT>(cx.prow1 + (in1[j] ? o1 : 0), b1[j]);
             }
         }
         // ---- the value right of each unit: first value of the right neighbour's unit, or an own load at the band / chunk edge
 #pragma unroll
         for (int32_t j = 0; j < NJ; j++)
         {
-            const int32_t off = (c0 + j) * CH + CPL * lane;
+            const int32_t off = (c0 + j) * kChunk + kCPL * lane;
             {
                 const int32_t o   = cx.sh0 + off;
                 const int32_t nbv = __shfl_down_sync(kFull, b0[j][0], 1);
-                const bool nb_in  = lane < 31 && (off + CPL) < cx.bw && (o + CPL) <= cx.lim0;
-                b0[j][CPL]        = nbv;
+                const bool nb_in  = lane < 31 && (off + kCPL) < cx.bw && (o + kCPL) <= cx.lim0;
+                b0[j][kCPL]       = nbv;
                 if (in0[j] && !nb_in)
-                    b0[j][CPL] = cx.prow0[o + CPL];
+                    b0[j][kCPL] = cx.prow0[o + kCPL];
             }
             if (TWO)
             {
                 const int32_t o   = cx.sh1 + off;
                 const int32_t nbv = __shfl_down_sync(kFull, b1[j][0], 1);
-                const bool nb_in  = lane < 31 && (off + CPL) < cx.bw && (o + CPL) <= cx.lim1;
-                b1[j][CPL]        = nbv;
+                const bool nb_in  = lane < 31 && (off + kCPL) < cx.bw && (o + kCPL) <= cx.lim1;
+                b1[j][kCPL]       = nbv;
                 if (in1[j] && !nb_in)
-                    b1[j][CPL] = cx.prow1[o + CPL];
+                    b1[j][kCPL] = cx.prow1[o + kCPL];
             }
         }
         // ---- candidates (get_scores(), cudapoa_nw_banded.cuh:104-156: the band test is per 4 cells) and the lane-local closure
 #pragma unroll
         for (int32_t j = 0; j < NJ; j++)
         {
-            const int32_t off = (c0 + j) * CH + CPL * lane;
+            const int32_t off = (c0 + j) * kChunk + kCPL * lane;
 #pragma unroll
-            for (int32_t i = 0; i < CPL; i++)
+            for (int32_t i = 0; i < kCPL; i++)
             {
                 // w holds read ^ base in every byte: a zero byte is a match (one logic op with a predicate result per cell)
                 const int32_t q  = ((w[j][i >> 2] & (0xffu << (8 * (i & 3)))) == 0u) ? cx.match : cx.mismatch;
@@ -328,7 +305,7 @@ __device__ __forceinline__ void row_group_v3(const RowCtx<ScoreT>& cx, const int
                 a[j][i] = v;
             }
 #pragma unroll
-            for (int32_t i = 1; i < CPL; i++)
+            for (int32_t i = 1; i < kCPL; i++)
                 a[j][i] = __viaddmax_s32(a[j][i - 1], gap, a[j][i]);
         }
     }
@@ -336,9 +313,9 @@ __device__ __forceinline__ void row_group_v3(const RowCtx<ScoreT>& cx, const int
 #pragma unroll
     for (int32_t j = 0; j < NJ; j++)
     {
-        const int32_t last_lane = min(31, (cx.bw - (c0 + j) * CH) / CPL - 1);
-        nbraw[j]                = __shfl_up_sync(kFull, a[j][CPL - 1], 1);
-        outv[j]                 = __shfl_sync(kFull, a[j][CPL - 1], last_lane);
+        const int32_t last_lane = min(31, (cx.bw - (c0 + j) * kChunk) / kCPL - 1);
+        nbraw[j]                = __shfl_up_sync(kFull, a[j][kCPL - 1], 1);
+        outv[j]                 = __shfl_sync(kFull, a[j][kCPL - 1], last_lane);
         s0l0[j]                 = __shfl_sync(kFull, a[j][0], 0);
         need[j]                 = __ballot_sync(kFull, lane > 0 && act[j] && nbraw[j] + gap > a[j][0]);
     }
@@ -349,31 +326,12 @@ __device__ __forceinline__ void row_group_v3(const RowCtx<ScoreT>& cx, const int
         leftv[j] = (lane == 0) ? cleft : nbraw[j];
         if (need[j] != 0u || cin + gap > s0l0[j])
         {
-            const int32_t last_lane = min(31, (cx.bw - (c0 + j) * CH) / CPL - 1);
-            const int32_t gl        = CPL * gap;
-            // A horizontal run crosses a lane boundary or enters from the chunk to the left. Right of the alignment path every
-            // cell is its left neighbour + gap: the run that enters the chunk dominates all of it (about half of the chunks of
-            // a wide band). The locally closed values satisfy a[i] >= a[i-1] + gap, so "every cell of the lane is dominated"
-            // is one comparison of the lane's last cell and the whole chunk is decided by one ballot; only the remaining
-            // chunks (the one the path crosses) run the max-plus prefix scan over the lanes.
-            const int32_t bound = cin + gl * (lane + 1);
-            if (GWB200_V3_PURE != 0 && __ballot_sync(kFull, act[j] && a[j][CPL - 1] > bound) == 0u)
-            {
-                const int32_t base = bound - gl;
-                if (lane != 0)
-                    leftv[j] = base;
-#pragma unroll
-                for (int32_t i = 0; i < CPL; i++)
-                    a[j][i] = base + (i + 1) * gap;
-                outv[j] = cin + gl * (last_lane + 1);
-            }
-            else
-            {
-                const int32_t L = chunk_scan<CPL>(a[j], cin, gap, lane);
-                if (lane != 0)
-                    leftv[j] = L;
-                outv[j] = __shfl_sync(kFull, a[j][CPL - 1], last_lane);
-            }
+            // a horizontal run crosses a lane boundary or enters from the chunk to the left: max-plus prefix scan over the lanes
+            const int32_t last_lane = min(31, (cx.bw - (c0 + j) * kChunk) / kCPL - 1);
+            const int32_t L         = chunk_scan(a[j], cin, gap, lane);
+            if (lane != 0)
+                leftv[j] = L;
+            outv[j] = __shfl_sync(kFull, a[j][kCPL - 1], last_lane);
         }
         cin   = static_cast<ScoreT>(outv[j]);
         cleft = cin;
@@ -382,51 +340,44 @@ __device__ __forceinline__ void row_group_v3(const RowCtx<ScoreT>& cx, const int
 #pragma unroll
     for (int32_t j = 0; j < NJ; j++)
     {
-        const int32_t off = (c0 + j) * CH + CPL * lane;
+        const int32_t off = (c0 + j) * kChunk + kCPL * lane;
         if (act[j])
         {
 #pragma unroll
-            for (int32_t i = 0; i < CPL; i++)
+            for (int32_t i = 0; i < kCPL; i++)
                 a[j][i] = static_cast<ScoreT>(a[j][i]);
-            unit_store<ScoreT, CPL>(cx.drow + off, static_cast<ScoreT>(leftv[j]), a[j]);
-            if (cx.grow != nullptr)
-                unit_store<ScoreT, CPL>(cx.grow + off, static_cast<ScoreT>(leftv[j]), a[j]);
+            unit_store<ScoreT>(cx.drow + off, static_cast<ScoreT>(leftv[j]), a[j]);
         }
     }
 }
 
 // The DP rows of needlemanWunschBanded (cudapoa_nw_banded.cuh:266-405) for one warp; everything before and after them (band
 // geometry, end cell, traceback) is in nw_banded_v3 below. Rows are written to `scores` (row r at r * stride) exactly once.
-template <typename ScoreT, typename SizeT, bool BULK>
+template <typename ScoreT, typename SizeT>
 __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const uint8_t* __restrict__ read, const Band<ScoreT>& B,
                            const int32_t band_width, const int32_t max_column, const int32_t gap, const int32_t mismatch, const int32_t match,
-                           int4* row_meta, uint8_t* pool, const int32_t pool_bytes, int4* srec, const int32_t max_group, const int32_t row_fence)
+                           int4* row_meta, uint8_t* pool, const int32_t pool_bytes, int4* srec, const int32_t max_group32)
 {
     constexpr int32_t kMin   = min_score_of<ScoreT>();
-    constexpr int32_t CPL    = V3Cells<ScoreT>::kCPL;
-    constexpr int32_t CH     = V3Cells<ScoreT>::kChunk;
-    constexpr int32_t GC     = 16 / CPL; // chunks per group: 16 cells per lane in flight
+    const int32_t max_group  = sizeof(ScoreT) == 2 ? 2 : max_group32; // chunks per straight-line group of a fast row
     const int32_t lane       = threadIdx.x & 31;
     const int32_t stride     = B.stride;
     ScoreT* const scores     = B.scores;
     const int32_t rowbytes   = stride * static_cast<int32_t>(sizeof(ScoreT));
-    const int32_t nchunks    = (band_width + CH - 1) / CH;
+    const int32_t nchunks    = (band_width + kChunk - 1) / kChunk;
     ScoreT* const ring       = reinterpret_cast<ScoreT*>(pool);
     // the host sizes the pool for at least two rows of the widest band (v3_pool_bytes): the rows always go through the ring, so
     // every row access of the fast path is a shared-memory access the compiler can see as one (no generic pointers)
     const int32_t R          = min(pool_bytes / rowbytes, 64);
     if (R < 2)
-        __trap(); // only reachable with the development override of the pool size
-    constexpr bool use_ring  = true;
-    constexpr bool bulk      = BULK;
+        __trap(); // guard: v3_pool_bytes never launches a pool this small
 
     // row 0: scores[j] = j * gap (:269-272), also into ring slot 0
     for (int32_t j = lane; j < stride; j += 32)
     {
         const ScoreT v = static_cast<ScoreT>(j * gap);
         scores[j]      = v;
-        if (use_ring)
-            ring[j] = v;
+        ring[j]        = v;
     }
 
     // ---- per-row records, prepared one 32-row group ahead (lane k <-> row r0 + 32 + k) and handed over through shared memory
@@ -441,7 +392,7 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
         const int32_t bsp1 = B.start(p1);
         const int32_t d0   = row - p0;
         const int32_t d1   = row - p1;
-        const bool fast    = use_ring && pc <= 2 && d0 < R && (pc < 2 || d1 < R);
+        const bool fast    = pc <= 2 && d0 < R && (pc < 2 || d1 < R);
         int4 r;
         r.x = bs | (base << 16) | (min(pc, 3) << 24) | ((fast ? 1 : 0) << 27);
         r.y = (bs - bsp0) | (min(band_width - kCPT, max_column - bsp0) << 16);
@@ -465,7 +416,7 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
 
     int32_t ring_slot = 0;
     ScoreT* rowp      = scores;
-    const int32_t off0 = CPL * lane; // local index of this lane's unit in chunk 0
+    const int32_t off0 = kCPL * lane; // local index of this lane's unit in chunk 0
 
     for (int32_t r0 = 1; r0 <= graph_count; r0 += 32)
     {
@@ -512,7 +463,6 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
             ring_slot          = (ring_slot + 1 == R) ? 0 : ring_slot + 1;
             rowp += stride;
             ScoreT* const srow = ring + ring_slot * stride;
-            ScoreT* const drow = use_ring ? srow : rowp; // where the lanes write the row
 
             int32_t local0, cin;
             if (rc.x & (1 << 27))
@@ -558,15 +508,14 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
                 local0 = (bs == 0) ? (pc == 0 ? gap : first) : kMin;
                 cin    = (pc == 0) ? 0 : first;
                 int32_t cleft = local0;
-                // Chunks are taken in groups of up to GC (row_group_v3): the candidate values and the lane-local closure of the
-                // chunks of a group are independent of each other, so their loads and arithmetic overlap; only the carry between
-                // chunks is sequential, and in the common case it is a scalar chain over values that are already known.
+                // Chunks are taken in groups of up to max_group (row_group_v3): the candidate values and the lane-local closure
+                // of the chunks of a group are independent of each other, so their loads and arithmetic overlap; only the carry
+                // between chunks is sequential, and in the common case it is a scalar chain over values that are already known.
                 RowCtx<ScoreT> cx;
                 cx.prow0 = prow0;
                 cx.prow1 = prow1;
                 cx.rd    = read + bs;
-                cx.drow  = drow;
-                cx.grow  = (!bulk && use_ring) ? rowp : nullptr;
+                cx.drow  = srow;
                 cx.sh0   = sh0;
                 cx.lim0  = lim0;
                 cx.sh1   = sh1;
@@ -591,9 +540,6 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
                 }
                 else
                 {
-                    if (GC >= 4 && max_group >= 4)
-                        for (; c0 + 4 <= nchunks; c0 += 4)
-                            row_group_v3<ScoreT, (GC >= 4 ? 4 : 1), false>(cx, c0, lane, cin, cleft);
                     if (max_group >= 2)
                         for (; c0 + 2 <= nchunks; c0 += 2)
                             row_group_v3<ScoreT, 2, false>(cx, c0, lane, cin, cleft);
@@ -610,34 +556,29 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
                 auto pred_index = [&](int32_t p) -> int32_t {
                     return (p == 0) ? rm.y : (p == 1 ? rm.z : static_cast<int32_t>(g.pos[g.in_edge(node_id, p)]) + 1);
                 };
-                if (bulk)
+                // Rows reach global memory by the bulk copies. A row with three or more predecessors that are all still in the
+                // ring needs none of that; otherwise everything older than the ring is complete once at most min(R, 4) - 1
+                // groups are pending (the wait makes the writes visible to the waiting thread -- and invalidates the L1 --, the
+                // warp barrier orders the other lanes behind it).
+                int32_t far = 0;
+                for (int32_t p = 0; p < pcf; p++)
+                    far |= (row - pred_index(p) >= R) ? 1 : 0;
+                if (far != 0)
                 {
-                    // Rows reach global memory by the bulk copies. A row with three or more predecessors that are all still in
-                    // the ring needs none of that; otherwise everything older than the ring is complete once at most
-                    // min(R, 4) - 1 groups are pending (the wait makes the writes visible to the waiting thread -- and
-                    // invalidates the L1 --, the warp barrier orders the other lanes behind it).
-                    int32_t far = 0;
-                    for (int32_t p = 0; p < pcf; p++)
-                        far |= (row - pred_index(p) >= R) ? 1 : 0;
-                    if (far != 0)
+                    if (lane == 0)
                     {
-                        if (lane == 0)
-                        {
-                            if (R >= 5)
-                                bulk_wait<3>();
-                            else if (R >= 3)
-                                bulk_wait<2>();
-                            else
-                                bulk_wait<1>();
-                            if (row_fence != 0)
-                                fence_async_all();
-                        }
-                        __syncwarp();
+                        if (R >= 5)
+                            bulk_wait<3>();
+                        else if (R >= 3)
+                            bulk_wait<2>();
+                        else
+                            bulk_wait<1>();
                     }
+                    __syncwarp();
                 }
                 auto pred_row_ptr = [&](int32_t pi) -> const ScoreT* {
                     const int32_t d = row - pi;
-                    if (use_ring && d < R)
+                    if (d < R)
                     {
                         int32_t sl = ring_slot - d;
                         if (sl < 0)
@@ -667,12 +608,12 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
                 const int32_t np = max(pcf, 1);
                 for (int32_t c = 0; c < nchunks; c++)
                 {
-                    const int32_t off = c * CH + off0;
+                    const int32_t off = c * kChunk + off0;
                     const bool active = off < band_width;
                     const int32_t rp  = bs + off;
-                    int32_t q[CPL];
+                    int32_t q[kCPL];
 #pragma unroll
-                    for (int32_t h = 0; h < CPL / 4; h++)
+                    for (int32_t h = 0; h < kCPL / 4; h++)
                     {
                         const uint32_t w0 = __ldg(reinterpret_cast<const uint32_t*>(read + rp + 4 * h));
                         q[4 * h + 0]      = (base == static_cast<int32_t>(w0 & 0xff)) ? match : mismatch;
@@ -680,9 +621,9 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
                         q[4 * h + 2]      = (base == static_cast<int32_t>((w0 >> 16) & 0xff)) ? match : mismatch;
                         q[4 * h + 3]      = (base == static_cast<int32_t>(w0 >> 24)) ? match : mismatch;
                     }
-                    int32_t s[CPL];
+                    int32_t s[kCPL];
 #pragma unroll
-                    for (int32_t i = 0; i < CPL; i++)
+                    for (int32_t i = 0; i < kCPL; i++)
                         s[i] = kMin;
                     for (int32_t p = 0; p < np; p++)
                     {
@@ -692,7 +633,7 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
                         const int32_t o    = (bs - bsp) + off;
                         const ScoreT* prow = pred_row_ptr(pi);
 #pragma unroll
-                        for (int32_t h = 0; h < CPL / 4; h++)
+                        for (int32_t h = 0; h < kCPL / 4; h++)
                         {
                             const int32_t oh = o + 4 * h;
                             if (active && oh <= lim)
@@ -711,20 +652,16 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
                         }
                     }
                     int32_t left;
-                    closure_seq<CPL>(s, cin, gap, lane, left);
+                    closure_seq(s, cin, gap, lane, left);
 #pragma unroll
-                    for (int32_t i = 0; i < CPL; i++)
+                    for (int32_t i = 0; i < kCPL; i++)
                         s[i] = static_cast<ScoreT>(s[i]);
                     if (lane == 0)
                         left = cleft;
                     if (active)
-                    {
-                        unit_store<ScoreT, CPL>(drow + off, left, s);
-                        if (!bulk && use_ring)
-                            unit_store<ScoreT, CPL>(rowp + off, left, s);
-                    }
-                    const int32_t last_lane = min(31, (band_width - c * CH) / CPL - 1);
-                    cin                     = __shfl_sync(kFull, s[CPL - 1], last_lane);
+                        unit_store<ScoreT>(srow + off, left, s);
+                    const int32_t last_lane = min(31, (band_width - c * kChunk) / kCPL - 1);
+                    cin                     = __shfl_sync(kFull, s[kCPL - 1], last_lane);
                     cleft                   = cin;
                 }
             }
@@ -736,50 +673,39 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
                 tl.y = static_cast<ScoreT>(kMin);
                 tl.z = static_cast<ScoreT>(kMin);
                 tl.w = static_cast<ScoreT>(kMin);
-                *reinterpret_cast<Vec4<ScoreT>*>(drow + band_width + 4 * lane) = tl;
-                if (!bulk && use_ring)
-                    *reinterpret_cast<Vec4<ScoreT>*>(rowp + band_width + 4 * lane) = tl;
+                *reinterpret_cast<Vec4<ScoreT>*>(srow + band_width + 4 * lane) = tl;
             }
-            if (bulk)
+            // generic-proxy writes of the row -> visible to the async proxy; the slot of the NEXT row (last used R rows before it)
+            // must have been read by its bulk copy before any lane writes it
+            fence_async_smem();
+            if (lane == 0)
             {
-                // generic-proxy writes of the row -> visible to the async proxy; the slot of the NEXT row (last used R rows
-                // before it) must have been read by its bulk copy before any lane writes it
-                fence_async_smem();
-                if (lane == 0)
-                {
-                    if (R >= 5)
-                        bulk_wait_read<3>();
-                    else if (R >= 3)
-                        bulk_wait_read<1>();
-                    else
-                        bulk_wait_read<0>();
-                }
-                __syncwarp();
-                if (lane == 0)
-                {
-                    bulk_store_s2g(rowp, srow, static_cast<uint32_t>(rowbytes));
-                    bulk_commit();
-                }
+                if (R >= 5)
+                    bulk_wait_read<3>();
+                else if (R >= 3)
+                    bulk_wait_read<1>();
+                else
+                    bulk_wait_read<0>();
             }
-            else
+            __syncwarp();
+            if (lane == 0)
             {
-                __syncwarp();
+                bulk_store_s2g(rowp, srow, static_cast<uint32_t>(rowbytes));
+                bulk_commit();
             }
         }
     }
-    if (bulk)
+    if (lane == 0)
     {
-        if (lane == 0)
-        {
-            bulk_wait<0>();
-            fence_async_all();
-        }
+        bulk_wait<0>();
+        fence_async_all();
     }
     __syncwarp();
 }
 
 // End-cell search + traceback of needlemanWunschBanded (cudapoa_nw_banded.cuh:407-549) for one warp, tile refilled by the lanes
-// with plain loads (the v2 routine; kept as the A/B partner of traceback_tma below). Returns the alignment length or a code.
+// with plain loads: the traceback for a pool smaller than the two tile buffers of traceback_tma below. Returns the alignment
+// length or a code.
 template <typename ScoreT, typename SizeT>
 __device__ int32_t traceback_plain(const Win<SizeT>& g, const int32_t graph_count, const uint8_t* read, const int32_t read_length,
                                    const Band<ScoreT>& B, SizeT* aln_graph, SizeT* aln_read, const int32_t band_width, const int32_t gap,
@@ -1340,7 +1266,10 @@ __device__ int32_t traceback_tma(const Win<SizeT>& g, const int32_t graph_count,
             loop_count++;
             if (i < t_lo || i > t_hi || j >= J0 + kTC || (j > 0 && j - 1 < J0))
                 ensure(i, j);
-            // ---- speculative run (see nw_banded_v2): lane k verifies step k of a run of "diagonal through the first predecessor"
+            // ---- speculative run: lane k assumes the previous k steps were all "diagonal through the first predecessor" (the
+            // first test of every step, :467-478), finds the row it would stand on by following k first-predecessor links
+            // (binary decomposition of k over the tile's pointer-doubling tables) and verifies its own step on the tile; the
+            // leading run of successful lanes is exactly what the serial loop would do for those steps, taken at once.
             {
                 int32_t pos = i - t_lo;
 #pragma unroll
@@ -1373,6 +1302,7 @@ __device__ int32_t traceback_tma(const Win<SizeT>& g, const int32_t graph_count,
                         ok                 = sij == sd + cost;
                     }
                 }
+                // the first step uses next_node_id, which must be the node of row i for the speculation to be the serial behaviour
                 const int32_t node0 = __shfl_sync(kFull, knode, 0);
                 uint32_t okmask     = __ballot_sync(kFull, ok);
                 if (node0 != next_node_id)
@@ -1426,7 +1356,8 @@ __device__ int32_t traceback_tma(const Win<SizeT>& g, const int32_t graph_count,
                         break;
                     }
                 }
-                // the reference uses next_node_id (= graph[prev_i - 1] of the previous step) here; kept, see nw_banded_v2
+                // the reference uses next_node_id (= graph[prev_i - 1] of the previous step) here; it equals graph[i - 1]
+                // whenever the previous step found a predecessor and is stale otherwise -- that behaviour is kept
                 const int32_t node_id = next_node_id;
                 int32_t nbase = m.w & 0xff, pc = pc_i, pred_i = m.y;
                 if (node_id != row_node)
@@ -1660,22 +1591,15 @@ __device__ void topsort_v3(const Win<SizeT>& g, const int32_t node_count, uint8_
     __syncwarp();
 }
 
-// needlemanWunschBanded (cudapoa_nw_banded.cuh:177-557) for one warp: band geometry as in nw_banded_v2, rows by dp_rows_v3,
-// end cell + traceback by traceback_tma (or traceback_plain when the pool is too small for the tile buffers).
-} // namespace poa
-} // namespace gwb200
-#include "poa_kernels_v4.cuh"
-namespace gwb200
-{
-namespace poa
-{
-
-template <typename ScoreT, typename SizeT, bool BULK, bool WAVE>
+// needlemanWunschBanded (cudapoa_nw_banded.cuh:177-557) for one warp: band geometry, rows by dp_rows_v3, end cell + traceback
+// by traceback_tma, or by traceback_plain for a pool smaller than two tile buffers. v3_pool_bytes never sizes one that small;
+// traceback_plain stays all the same because without it ptxas lays out the kernel differently and C2 / C3 of bench.py measured
+// 4-7 % slower on an H100.
+template <typename ScoreT, typename SizeT>
 __device__ int32_t nw_banded_v3(const Win<SizeT>& g, int32_t graph_count, const uint8_t* read, int32_t read_length, ScoreT* scores,
                                 float max_buffer_size, SizeT* aln_graph, SizeT* aln_read, int32_t band_width, int32_t gap, int32_t mismatch,
                                 int32_t match, int32_t rerun, const bool Adaptive, unsigned long long& cells, int4* row_meta, uint8_t* pool,
-                                int32_t pool_bytes, unsigned long long* timers, V3Shared* sh, const int32_t tb_mode, const int32_t wavefront, const int32_t max_group,
-                                const int32_t row_fence)
+                                int32_t pool_bytes, unsigned long long* timers, V3Shared* sh, const int32_t max_group32)
 {
     GWB200_TIMER_START();
     const float gradient     = __fdividef(static_cast<float>(read_length + 1), static_cast<float>(graph_count + 1));
@@ -1717,19 +1641,11 @@ __device__ int32_t nw_banded_v3(const Win<SizeT>& g, int32_t graph_count, const 
         cells += static_cast<unsigned long long>(graph_count) * static_cast<unsigned long long>(band_width);
 
     Band<ScoreT> B{scores, band_width, band_shift, max_column, band_width + kRightPad, gradient};
-    bool done = false;
-    if constexpr (WAVE && sizeof(ScoreT) == 4)
-    {
-        if (wavefront != 0 && B.start(graph_count) < 65536)
-            done = dp_rows_v4<ScoreT, SizeT>(g, graph_count, read, B, band_width, max_column, gap, mismatch, match, row_meta, pool, pool_bytes,
-                                             sh->rec[0]);
-    }
-    if (!done)
-        dp_rows_v3<ScoreT, SizeT, BULK>(g, graph_count, read, B, band_width, max_column, gap, mismatch, match, row_meta, pool, pool_bytes, sh->rec[0],
-                                        max_group, row_fence);
+    dp_rows_v3<ScoreT, SizeT>(g, graph_count, read, B, band_width, max_column, gap, mismatch, match, row_meta, pool, pool_bytes, sh->rec[0],
+                              max_group32);
     GWB200_TIMER_LAP(0);
     int32_t result;
-    if (tb_mode != 0 && pool_bytes >= TileBuf<ScoreT>::kBytes * 2)
+    if (pool_bytes >= TileBuf<ScoreT>::kBytes * 2)
         result = traceback_tma<ScoreT, SizeT>(g, graph_count, read, read_length, B, aln_graph, aln_read, band_width, gap, mismatch, match, rerun,
                                               Adaptive, row_meta, pool, sh->tile_bar, timers, t_ph__);
     else
@@ -1740,7 +1656,7 @@ __device__ int32_t nw_banded_v3(const Win<SizeT>& g, int32_t graph_count, const 
 }
 
 // One window from the backbone to the consensus / MSA (cudapoa_kernels.cuh:200-541) on one warp.
-template <typename ScoreT, typename SizeT, bool BULK, bool WAVE>
+template <typename ScoreT, typename SizeT>
 __device__ void process_window_v3(const DeviceParams& P, const V2Extra& X, const V3Extra& Y, const int32_t w, uint8_t* pool, V3Shared* sh)
 {
     const bool MSA      = P.msa != 0;
@@ -1846,9 +1762,9 @@ __device__ void process_window_v3(const DeviceParams& P, const V2Extra& X, const
                 int32_t rerun       = 0;
                 for (int32_t attempt = 0; attempt < 2; attempt++)
                 {
-                    alen = nw_banded_v3<ScoreT, SizeT, BULK, WAVE>(g, node_count, sequence, seq_len, scores, banded_buffer_size, aln_graph, aln_read,
-                                                             P.band_width, P.gap, P.mismatch, P.match, rerun, adaptive, cells, row_meta, pool,
-                                                             X.pool_bytes, timers, sh, Y.tb_tma, Y.wavefront, Y.max_group, Y.row_fence);
+                    alen = nw_banded_v3<ScoreT, SizeT>(g, node_count, sequence, seq_len, scores, banded_buffer_size, aln_graph, aln_read,
+                                                       P.band_width, P.gap, P.mismatch, P.match, rerun, adaptive, cells, row_meta, pool,
+                                                       X.pool_bytes, timers, sh, Y.max_group32);
                     if (!adaptive || attempt == 1 || !(alen == kShiftLeft || alen == kShiftRight))
                         break;
                     rerun = alen; // rerun with extended and shifted band (cudapoa_kernels.cuh:374-396)
@@ -1932,8 +1848,8 @@ __device__ void process_window_v3(const DeviceParams& P, const V2Extra& X, const
 }
 
 // Persistent grid: one warp per CTA, every CTA pulls window indices from the batch's work counter until none is left.
-template <typename ScoreT, typename SizeT, bool BULK, bool WAVE>
-__global__ void __launch_bounds__(32, (WAVE ? 8 : (sizeof(ScoreT) == 4 ? 12 : 16))) poa_window_kernel_v3(const DeviceParams P, const V2Extra X, const V3Extra Y)
+template <typename ScoreT, typename SizeT>
+__global__ void __launch_bounds__(32, (sizeof(ScoreT) == 4 ? 12 : 16)) poa_window_kernel_v3(const DeviceParams P, const V2Extra X, const V3Extra Y)
 {
     extern __shared__ __align__(16) uint8_t pool[];
     __shared__ __align__(16) V3Shared sh;
@@ -1955,7 +1871,7 @@ __global__ void __launch_bounds__(32, (WAVE ? 8 : (sizeof(ScoreT) == 4 ? 12 : 16
         w = __shfl_sync(kFull, w, 0);
         if (w >= P.n_windows)
             break;
-        process_window_v3<ScoreT, SizeT, BULK, WAVE>(P, X, Y, w, pool, &sh);
+        process_window_v3<ScoreT, SizeT>(P, X, Y, w, pool, &sh);
     }
 }
 

@@ -245,10 +245,7 @@ class CudaPoaBatch:
         out = np.zeros(8, dtype=np.uint64)
         check(lib().gwb200_poa_batch_get_timers(self._h, out.ctypes.data))
         names = ["dp_rows", "end_cell", "traceback", "add_alignment", "topsort", "consensus"]
-        d = dict(zip(names, [int(x) for x in out[:6]]))
-        if out[6] or out[7]:  # row-level probes of a -DGWB200_ROW_PROFILE build
-            d["aux6"], d["aux7"] = int(out[6]), int(out[7])
-        return d
+        return dict(zip(names, [int(x) for x in out[:6]]))
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:

@@ -227,8 +227,8 @@ def test_int32_sizes_long_window_vs_reference():
 
 
 def test_static_band_512_and_128_vs_reference():
-    """Other kernel configurations: 1 chunk (band 128, one warp), 3 chunks (band 384: three of four warps take part in the rows)
-    and 4 chunks (band 512, four warps x one chunk)."""
+    """Other band widths of the v3 rows (256 columns per chunk): band 128 leaves lanes of its one chunk idle, band 384 ends in a
+    half chunk, band 512 fills two chunks (one straight-line group of int16 rows)."""
     from genomeworks_b200 import cudapoa, synth
     win_nseq, seq_len, data = synth.poa_windows(40, 900, 10, 20, 12, 12, seed0=555, max_read_len=1024)
     for bw in (128, 384, 512):
@@ -236,6 +236,18 @@ def test_static_band_512_and_128_vs_reference():
         ours = run_ours(win_nseq, seq_len, data, cfg)
         ref = reference("static_band/%d" % bw, win_nseq, seq_len, data, 1024, 16, bw, 1)
         assert_same_as_reference(ours, ref, "reference bw=%d" % bw)
+
+
+def test_static_band_2048_first_generation_kernel_vs_oracle(device_fdiv):
+    """A band wider than the widest adaptive band (1536) runs the first-generation kernel (poa_kernels.cuh)."""
+    from genomeworks_b200 import cudapoa, synth
+    win_nseq, seq_len, data = synth.poa_windows(24, 900, 10, 10, 5, 5, seed0=2048, max_read_len=1024)
+    cfg = cudapoa.make_config(1024, 16, 2048, "static_band")
+    ours = run_ours(win_nseq, seq_len, data, cfg)
+    assert (ours["status"] == 0).all()
+    orc = ol.poa_run(synth.split_windows(win_nseq, seq_len, data), _cfg8(cfg))
+    assert_same_consensus(ours, orc, "oracle")
+    assert ours["cells"] == int(orc["cells"].sum())
 
 
 # ---- traceback band modes (cudapoa_nw_tb_banded.cuh): static / adaptive band with a trace matrix and a score ring ----

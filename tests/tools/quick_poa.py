@@ -1,5 +1,5 @@
-"""Development aid: time a POA config (ours, optional v1 A/B via GWB200_POA_KERNEL=v1) and print per-phase cycle shares.
-usage: quick_poa.py {c2|c3} [n_windows] [--ref] [--factor F] [--len L] [--msa] [--band-mode NAME (c2 only)]   (env GWB200_POA_WARPS / GWB200_POA_POOL_KB: kernel experiments)"""
+"""Development aid: time a POA config, print per-phase cycle shares and a digest of the consensus.
+usage: quick_poa.py {c2|c3} [n_windows] [--ref] [--factor F] [--len L] [--msa] [--band-mode NAME (c2 only)]"""
 import os
 import sys
 import time
@@ -12,7 +12,7 @@ from genomeworks_b200 import cudapoa, synth
 import ref_lib
 
 which = sys.argv[1] if len(sys.argv) > 1 else "c2"
-n = int(sys.argv[2]) if len(sys.argv) > 2 else (1024 if which == "c2" else 132)
+n = int(sys.argv[2]) if len(sys.argv) > 2 and not sys.argv[2].startswith("--") else (1024 if which == "c2" else 132)
 if which == "c2":
     win_nseq, seq_len, data = synth.poa_windows(n, 1000, 16, 20, 10, 10, seed0=1000, max_read_len=1024)
     bm = sys.argv[sys.argv.index("--band-mode") + 1] if "--band-mode" in sys.argv else "static_band"  # e.g. static_band_traceback
@@ -34,7 +34,8 @@ MSA = "--msa" in sys.argv
 if MSA and which != "c2":
     mem += int(n * 1.2e6 * 32)  # MSA rows + per-read node paths
 b = cudapoa.CudaPoaBatch(cfg.max_sequences_per_poa, cfg.max_sequence_size, mem, output_type="msa" if MSA else "consensus", config=cfg)
-print("kernel", os.environ.get("GWB200_POA_KERNEL", "v3"), "max_poas", b.max_poas, "resident", b.resident_windows, flush=True)
+kernel = "tb" if cfg.band_mode in (cudapoa.BAND_MODES["static_band_traceback"], cudapoa.BAND_MODES["adaptive_band_traceback"]) else "v3"
+print("kernel", kernel, "max_poas", b.max_poas, "resident", b.resident_windows, flush=True)
 for it in range(3):
     b.reset()
     b.add_poa_groups_flat(win_nseq, seq_len, data)
@@ -51,10 +52,7 @@ for it in range(3):
     print("ours: generate+get %.1f ms, kernel %.2f ms, cells %.3e, ok=%d  -> %.0f windows/s" % ((t2 - t1) * 1e3, b.last_kernel_ms(), b.last_cells(),
                                                                                              int((st == 0).sum()), n / (b.last_kernel_ms() / 1e3)), flush=True)
 tm = b.get_timers()
-aux = {k: tm.pop(k) for k in ("aux6", "aux7") if k in tm}
 tot = max(1, sum(tm.values()))
-if aux:
-    print("row probes (share of dp_rows):", {k: "%.1f%%" % (100.0 * v / max(1, tm["dp_rows"])) for k, v in aux.items()})
 print("phase shares:", {k: "%.1f%%" % (100.0 * v / tot) for k, v in tm.items()}, "cycles/window %.3e" % (tot / n), flush=True)
 if MSA:
     print("msa: rows of window 0:", len(msa[0]), "columns:", len(msa[0][0]) if msa[0] else 0)
