@@ -732,10 +732,7 @@ static int poa_batch_create_impl(gwb200_poa_batch** out, int32_t device_id, void
     cudaEventCreate(&b->ev0);
     cudaEventCreate(&b->ev1);
     if (b->kernel == PoaKernel::v3)
-    {
         b->X.pool_bytes = v3_pool_bytes(b);
-        b->Y.max_group32 = 1;
-    }
     else if (b->kernel == PoaKernel::tb)
         b->X.pool_bytes = tb_pool_bytes(b);
     gwb200_poa_batch_reset(b);

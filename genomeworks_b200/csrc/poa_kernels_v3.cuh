@@ -6,14 +6,14 @@
 //   scheduling   one warp owns one window from the first read to the consensus; the grid is persistent (resident CTAs pull
 //                window indices from an atomic counter), so every resident warp always has work of its own, no CTA barrier
 //                exists anywhere, and batches that are not a multiple of the residency do not pay a wave quantum.
-//   DP rows      every lane owns 8 cells of the row per chunk of 256 columns (int16: one 16-byte unit, the rows leave as 8-wide
-//                vectors; int32: two units), so that the per-chunk costs are paid once per 256 columns. Chunks are taken left
-//                to right with the horizontal carry passed on directly (no two-phase fold). The predecessor rows are read as
-//                LDS.128 from a shared-memory ring of the most recent rows (always: the host sizes the pool for it), the
-//                value beyond the unit comes from the right neighbour by shuffle (no bank-conflicting scalar load), the
-//                substitution test is one xor per four read characters and one predicate-producing logic op per cell,
-//                per-row graph metadata is prepared 32 rows ahead by the lanes and handed over as one 16-byte shared-memory
-//                record per row.
+//   DP rows      fast rows (at most two predecessors, both in the ring) run as strips: lane k owns the band_width / 32
+//                contiguous cells [k S, (k + 1) S) of the row, walks them in 4-cell units with the lane-local closure carried
+//                across the whole strip, and the row needs one carry resolution across the lanes (strip_row_v3). Bands of one
+//                chunk (<= 256), int32 rows of a 1024 band (whose strips would all sit in the same shared-memory banks) and the
+//                general rows take 256 columns at a time with 8 cells per lane. The predecessor rows are read from a shared-memory ring of the most recent rows
+//                (always: the host sizes the pool for it), the substitution test is one xor per four read characters and one
+//                predicate-producing logic op per cell, per-row graph metadata is prepared 32 rows ahead by the lanes and handed
+//                over as one 16-byte shared-memory record per row.
 //   write-back   the finished row is written once into its ring slot and leaves for HBM as ONE bulk asynchronous copy
 //                (cp.async.bulk.global.shared::cta, bulk-group completion) issued by lane 0: the lanes issue no global
 //                stores in the row loop, and the ring slot is reused only after its bulk read has completed.
@@ -85,10 +85,6 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t pari
 struct V3Extra
 {
     int32_t* work_counter; // next window index (persistent grid), reset by the host before every launch
-    // chunks per straight-line group of a fast row with 32-bit scores: 1 (8 cells per lane in flight; 16-bit rows always take
-    // groups of 2). A kernel argument rather than a constant: with the 2-chunk groups compiled out, ptxas lays out the 32-bit
-    // kernel differently and C3 of bench.py measured 5 % slower on an H100
-    int32_t max_group32;
 };
 
 // Static shared memory of the v3 kernel that is not part of the pool
@@ -100,8 +96,8 @@ struct V3Shared
     uint32_t pad_[2];
 };
 
-// cells per lane and chunk: 8 (int16: one 16-byte unit, int32: two), so that the per-chunk costs -- neighbour shuffle, carry
-// shuffles and ballot, addressing, band tests -- are paid once per 256 columns
+// general rows (hubs, predecessors outside the ring): cells per lane and chunk, 8 (int16: one 16-byte unit, int32: two), so that
+// the per-chunk costs -- carry shuffles and ballot, addressing, band tests -- are paid once per 256 columns
 constexpr int32_t kCPL   = 8;
 constexpr int32_t kChunk = 32 * kCPL; // columns per chunk
 
@@ -190,7 +186,7 @@ __device__ __forceinline__ void closure_seq(int32_t (&s)[kCPL], int32_t cin, int
     left = L;
 }
 
-// The max-plus prefix scan of one chunk (the grouped row code below needs it for a minority of its chunks)
+// The max-plus prefix scan of one chunk (row_chunk_v3 needs it for a minority of its chunks)
 __device__ __forceinline__ int32_t chunk_scan(int32_t (&a)[kCPL], const int32_t cin, const int32_t gap, const int32_t lane)
 {
     const int32_t gl = kCPL * gap;
@@ -211,7 +207,7 @@ __device__ __forceinline__ int32_t chunk_scan(int32_t (&a)[kCPL], const int32_t 
     return L;
 }
 
-// What a group of chunks needs to know about its row (fast rows: at most two predecessors, both in the ring)
+// What a chunk needs to know about its row (fast rows: at most two predecessors, both in the ring)
 template <typename ScoreT>
 struct RowCtx
 {
@@ -224,131 +220,227 @@ struct RowCtx
     uint32_t base4; // the row's base in every byte
 };
 
-// NJ consecutive chunks of one row, starting at chunk c0 (all of them exist: c0 + NJ <= number of chunks). Straight-line code:
-// every load of the group is issued before the first dependent instruction needs it. cin: carry into the first chunk (closed
-// value of the cell left of it), cleft: what is stored in that cell's place; both are updated for the next group.
-template <typename ScoreT, int32_t NJ, bool TWO>
-__device__ __forceinline__ void row_group_v3(const RowCtx<ScoreT>& cx, const int32_t c0, const int32_t lane, int32_t& cin, int32_t& cleft)
+// Chunk c (256 columns, 8 cells per lane) of a fast row. cin: carry into the chunk (closed value of the cell left of it), cleft:
+// what is stored in that cell's place; both are updated for the next chunk.
+template <typename ScoreT, bool TWO>
+__device__ __forceinline__ void row_chunk_v3(const RowCtx<ScoreT>& cx, const int32_t c, const int32_t lane, int32_t& cin, int32_t& cleft)
 {
     constexpr int32_t kMin = min_score_of<ScoreT>();
     const int32_t gap      = cx.gap;
-    int32_t a[NJ][kCPL];
-    int32_t nbraw[NJ], outv[NJ], s0l0[NJ], leftv[NJ];
-    uint32_t need[NJ];
-    bool act[NJ];
+    const int32_t off      = c * kChunk + kCPL * lane;
+    const bool act         = off < cx.bw;
+    int32_t a[kCPL];
     {
-        // ---- loads: read characters and the predecessors' units of every chunk
-        uint32_t w[NJ][kCPL / 4];
-        int32_t b0[NJ][kCPL + 1], b1[TWO ? NJ : 1][kCPL + 1];
-        bool in0[NJ], in1[TWO ? NJ : 1];
+        // ---- loads: read characters and the predecessors' units
+        uint32_t w[kCPL / 4];
+        int32_t b0[kCPL + 1], b1[kCPL + 1];
 #pragma unroll
-        for (int32_t j = 0; j < NJ; j++)
+        for (int32_t h = 0; h < kCPL / 4; h++)
+            w[h] = __ldg(reinterpret_cast<const uint32_t*>(cx.rd + off + 4 * h)) ^ cx.base4;
+        const int32_t o0 = cx.sh0 + off;
+        const bool in0   = act && o0 <= cx.lim0;
+        // lanes outside the predecessor's band load its first unit instead: their values are discarded by ok0 below
+        unit_load<ScoreT>(cx.prow0 + (in0 ? o0 : 0), b0);
+        const int32_t o1 = cx.sh1 + off;
+        bool in1         = false;
+        if (TWO)
         {
-            const int32_t off = (c0 + j) * kChunk + kCPL * lane;
-            act[j]            = off < cx.bw;
-#pragma unroll
-            for (int32_t h = 0; h < kCPL / 4; h++)
-                w[j][h] = __ldg(reinterpret_cast<const uint32_t*>(cx.rd + off + 4 * h)) ^ cx.base4;
-            const int32_t o = cx.sh0 + off;
-            in0[j]          = act[j] && o <= cx.lim0;
-            // lanes outside the predecessor's band load its first unit instead: their values are discarded by ok0 below
-            unit_load<ScoreT>(cx.prow0 + (in0[j] ? o : 0), b0[j]);
-            if (TWO)
-            {
-                const int32_t o1 = cx.sh1 + off;
-                in1[j]           = act[j] && o1 <= cx.lim1;
-                unit_load<ScoreT>(cx.prow1 + (in1[j] ? o1 : 0), b1[j]);
-            }
+            in1 = act && o1 <= cx.lim1;
+            unit_load<ScoreT>(cx.prow1 + (in1 ? o1 : 0), b1);
         }
-        // ---- the value right of each unit: first value of the right neighbour's unit, or an own load at the band / chunk edge
-#pragma unroll
-        for (int32_t j = 0; j < NJ; j++)
+        // ---- the value right of the unit: first value of the right neighbour's unit, or an own load at the band / chunk edge
         {
-            const int32_t off = (c0 + j) * kChunk + kCPL * lane;
-            {
-                const int32_t o   = cx.sh0 + off;
-                const int32_t nbv = __shfl_down_sync(kFull, b0[j][0], 1);
-                const bool nb_in  = lane < 31 && (off + kCPL) < cx.bw && (o + kCPL) <= cx.lim0;
-                b0[j][kCPL]       = nbv;
-                if (in0[j] && !nb_in)
-                    b0[j][kCPL] = cx.prow0[o + kCPL];
-            }
-            if (TWO)
-            {
-                const int32_t o   = cx.sh1 + off;
-                const int32_t nbv = __shfl_down_sync(kFull, b1[j][0], 1);
-                const bool nb_in  = lane < 31 && (off + kCPL) < cx.bw && (o + kCPL) <= cx.lim1;
-                b1[j][kCPL]       = nbv;
-                if (in1[j] && !nb_in)
-                    b1[j][kCPL] = cx.prow1[o + kCPL];
-            }
+            const int32_t nbv = __shfl_down_sync(kFull, b0[0], 1);
+            const bool nb_in  = lane < 31 && (off + kCPL) < cx.bw && (o0 + kCPL) <= cx.lim0;
+            b0[kCPL]          = nbv;
+            if (in0 && !nb_in)
+                b0[kCPL] = cx.prow0[o0 + kCPL];
+        }
+        if (TWO)
+        {
+            const int32_t nbv = __shfl_down_sync(kFull, b1[0], 1);
+            const bool nb_in  = lane < 31 && (off + kCPL) < cx.bw && (o1 + kCPL) <= cx.lim1;
+            b1[kCPL]          = nbv;
+            if (in1 && !nb_in)
+                b1[kCPL] = cx.prow1[o1 + kCPL];
         }
         // ---- candidates (get_scores(), cudapoa_nw_banded.cuh:104-156: the band test is per 4 cells) and the lane-local closure
 #pragma unroll
-        for (int32_t j = 0; j < NJ; j++)
+        for (int32_t i = 0; i < kCPL; i++)
         {
-            const int32_t off = (c0 + j) * kChunk + kCPL * lane;
-#pragma unroll
-            for (int32_t i = 0; i < kCPL; i++)
+            // w holds read ^ base in every byte: a zero byte is a match (one logic op with a predicate result per cell)
+            const int32_t q  = ((w[i >> 2] & (0xffu << (8 * (i & 3)))) == 0u) ? cx.match : cx.mismatch;
+            const bool ok0   = (i < 4) ? in0 : (in0 && (o0 + 4) <= cx.lim0);
+            const int32_t t0 = static_cast<ScoreT>(__viaddmax_s32(b0[i + 1], gap, b0[i] + q));
+            int32_t v        = ok0 ? t0 : kMin;
+            if (TWO)
             {
-                // w holds read ^ base in every byte: a zero byte is a match (one logic op with a predicate result per cell)
-                const int32_t q  = ((w[j][i >> 2] & (0xffu << (8 * (i & 3)))) == 0u) ? cx.match : cx.mismatch;
-                const bool ok0   = (i < 4) ? in0[j] : (in0[j] && (cx.sh0 + off + 4) <= cx.lim0);
-                const int32_t t0 = static_cast<ScoreT>(__viaddmax_s32(b0[j][i + 1], gap, b0[j][i] + q));
-                int32_t v        = ok0 ? t0 : kMin;
-                if (TWO)
-                {
-                    const bool ok1   = (i < 4) ? in1[j] : (in1[j] && (cx.sh1 + off + 4) <= cx.lim1);
-                    const int32_t t1 = static_cast<ScoreT>(__viaddmax_s32(b1[j][i + 1], gap, b1[j][i] + q));
-                    v                = ok1 ? max(v, t1) : v;
-                }
-                a[j][i] = v;
+                const bool ok1   = (i < 4) ? in1 : (in1 && (o1 + 4) <= cx.lim1);
+                const int32_t t1 = static_cast<ScoreT>(__viaddmax_s32(b1[i + 1], gap, b1[i] + q));
+                v                = ok1 ? max(v, t1) : v;
             }
-#pragma unroll
-            for (int32_t i = 1; i < kCPL; i++)
-                a[j][i] = __viaddmax_s32(a[j][i - 1], gap, a[j][i]);
+            a[i] = v;
         }
-    }
-    // ---- what the carry resolution needs from the neighbours (independent of the carry: issued for all chunks at once)
 #pragma unroll
-    for (int32_t j = 0; j < NJ; j++)
-    {
-        const int32_t last_lane = min(31, (cx.bw - (c0 + j) * kChunk) / kCPL - 1);
-        nbraw[j]                = __shfl_up_sync(kFull, a[j][kCPL - 1], 1);
-        outv[j]                 = __shfl_sync(kFull, a[j][kCPL - 1], last_lane);
-        s0l0[j]                 = __shfl_sync(kFull, a[j][0], 0);
-        need[j]                 = __ballot_sync(kFull, lane > 0 && act[j] && nbraw[j] + gap > a[j][0]);
+        for (int32_t i = 1; i < kCPL; i++)
+            a[i] = __viaddmax_s32(a[i - 1], gap, a[i]);
     }
-    // ---- carries, chunk by chunk (uniform control flow)
-#pragma unroll
-    for (int32_t j = 0; j < NJ; j++)
+    // ---- carry
+    const int32_t last_lane = min(31, (cx.bw - c * kChunk) / kCPL - 1);
+    const int32_t nbraw     = __shfl_up_sync(kFull, a[kCPL - 1], 1);
+    int32_t outv            = __shfl_sync(kFull, a[kCPL - 1], last_lane);
+    const int32_t s0l0      = __shfl_sync(kFull, a[0], 0);
+    const uint32_t need     = __ballot_sync(kFull, lane > 0 && act && nbraw + gap > a[0]);
+    int32_t leftv           = (lane == 0) ? cleft : nbraw;
+    if (need != 0u || cin + gap > s0l0)
     {
-        leftv[j] = (lane == 0) ? cleft : nbraw[j];
-        if (need[j] != 0u || cin + gap > s0l0[j])
+        // a horizontal run crosses a lane boundary or enters from the chunk to the left: max-plus prefix scan over the lanes
+        const int32_t L = chunk_scan(a, cin, gap, lane);
+        if (lane != 0)
+            leftv = L;
+        outv = __shfl_sync(kFull, a[kCPL - 1], last_lane);
+    }
+    cin   = static_cast<ScoreT>(outv);
+    cleft = cin;
+    // ---- store
+    if (act)
+    {
+#pragma unroll
+        for (int32_t i = 0; i < kCPL; i++)
+            a[i] = static_cast<ScoreT>(a[i]);
+        unit_store<ScoreT>(cx.drow + off, static_cast<ScoreT>(leftv), a);
+    }
+}
+
+// 4 consecutive cells <-> int32 values (band starts and strips are multiples of 4 cells: 8-byte aligned for int16, 16 for int32)
+template <typename ScoreT>
+__device__ __forceinline__ void quad_load(const ScoreT* p, int32_t (&b)[4])
+{
+    const Vec4<ScoreT> v = *reinterpret_cast<const Vec4<ScoreT>*>(p);
+    b[0]                 = v.x;
+    b[1]                 = v.y;
+    b[2]                 = v.z;
+    b[3]                 = v.w;
+}
+template <typename ScoreT>
+__device__ __forceinline__ void quad_store(ScoreT* p, int32_t x, int32_t y, int32_t z, int32_t w)
+{
+    Vec4<ScoreT> v;
+    v.x                                  = static_cast<ScoreT>(x);
+    v.y                                  = static_cast<ScoreT>(y);
+    v.z                                  = static_cast<ScoreT>(z);
+    v.w                                  = static_cast<ScoreT>(w);
+    *reinterpret_cast<Vec4<ScoreT>*>(p) = v;
+}
+
+// One fast row (at most two predecessors, both in the ring) as strips: lane k computes the S = band_width / 32 contiguous cells
+// [k S, (k + 1) S) of the band (a multiple of 4: bands are multiples of 128), so that a row of any width needs one carry
+// resolution across the lanes instead of one per 256 columns.
+//   pass 1   left to right over the strip's 4-cell units (a runtime loop: the row loop has to stay resident in the instruction
+//            caches): candidates of get_scores() (cudapoa_nw_banded.cuh:104-156, band test per 4 cells), the lane-local closure
+//            s[c] = max(h[c], s[c-1] + gap) without carry-in, and the store into the ring slot. The value right of a unit is the
+//            first value of the next unit, which is the next iteration's load.
+//   carry    L, the closed value left of each strip: the left neighbour's strip end, unless the ballot finds a lane whose first
+//            cell it improves -- then the max-plus prefix scan over the strip ends.
+//   pass 2   s[c] = max(s[c], L + (c + 1) gap) from the strip start up to the first cell it does not improve: from there on the
+//            lane-local closure dominates. The unit at the strip start is rewritten in any case: it holds the value left of it.
+// The layout of the slot is that of every row: local column 0 = the cell left of the band (local0), cell c at local c + 1, so a
+// lane's unit store at its strip start holds the closed value left of the strip. Returns the closed value of the strip's last cell.
+// o0 / o1: offsets of the strip start in the predecessor rows; rd, drow: read and ring slot at the strip start.
+template <typename ScoreT, bool TWO>
+__device__ __forceinline__ int32_t strip_row_v3(const ScoreT* prow0, int32_t o0, const int32_t lim0, const ScoreT* prow1, int32_t o1,
+                                                const int32_t lim1, const uint8_t* rd, const uint32_t base4, ScoreT* drow, const int32_t S,
+                                                const int32_t cin, const int32_t local0, const int32_t gap, const int32_t match,
+                                                const int32_t mismatch, const int32_t lane)
+{
+    constexpr int32_t kMin = min_score_of<ScoreT>();
+    // units outside a predecessor's band load its first unit instead: their values are discarded by the band test below
+    int32_t b0[4], b1[4];
+    quad_load<ScoreT>(prow0 + (o0 <= lim0 ? o0 : 0), b0);
+    if (TWO)
+        quad_load<ScoreT>(prow1 + (o1 <= lim1 ? o1 : 0), b1);
+    uint32_t w = __ldg(reinterpret_cast<const uint32_t*>(rd));
+    int32_t s3 = 0, k0 = 0;
+#pragma unroll 1
+    for (int32_t j = 0; j < S; j += 4)
+    {
+        // the next unit of the predecessor rows: within the row whenever this unit is in its band (lim <= band_width - 4)
+        const bool in0 = o0 <= lim0;
+        int32_t n0[4], n1[4];
+        quad_load<ScoreT>(prow0 + (in0 ? o0 + 4 : 0), n0);
+        bool in1 = false;
+        if (TWO)
         {
-            // a horizontal run crosses a lane boundary or enters from the chunk to the left: max-plus prefix scan over the lanes
-            const int32_t last_lane = min(31, (cx.bw - (c0 + j) * kChunk) / kCPL - 1);
-            const int32_t L         = chunk_scan(a[j], cin, gap, lane);
-            if (lane != 0)
-                leftv[j] = L;
-            outv[j] = __shfl_sync(kFull, a[j][kCPL - 1], last_lane);
+            in1 = o1 <= lim1;
+            quad_load<ScoreT>(prow1 + (in1 ? o1 + 4 : 0), n1);
         }
-        cin   = static_cast<ScoreT>(outv[j]);
-        cleft = cin;
-    }
-    // ---- stores
+        // x holds read ^ base in every byte: a zero byte is a match (one logic op with a predicate result per cell)
+        const uint32_t x = w ^ base4;
+        w                = __ldg(reinterpret_cast<const uint32_t*>(rd + min(j + 4, S - 4)));
+        int32_t v[4];
 #pragma unroll
-    for (int32_t j = 0; j < NJ; j++)
-    {
-        const int32_t off = (c0 + j) * kChunk + kCPL * lane;
-        if (act[j])
+        for (int32_t i = 0; i < 4; i++)
         {
-#pragma unroll
-            for (int32_t i = 0; i < kCPL; i++)
-                a[j][i] = static_cast<ScoreT>(a[j][i]);
-            unit_store<ScoreT>(cx.drow + off, static_cast<ScoreT>(leftv[j]), a[j]);
+            const int32_t q  = ((x & (0xffu << (8 * i))) == 0u) ? match : mismatch;
+            const int32_t t0 = static_cast<ScoreT>(__viaddmax_s32(i < 3 ? b0[i + 1] : n0[0], gap, b0[i] + q));
+            v[i]             = in0 ? t0 : kMin;
+            if (TWO)
+            {
+                const int32_t t1 = static_cast<ScoreT>(__viaddmax_s32(i < 3 ? b1[i + 1] : n1[0], gap, b1[i] + q));
+                v[i]             = in1 ? max(v[i], t1) : v[i];
+            }
         }
+        if (j != 0)
+            v[0] = __viaddmax_s32(s3, gap, v[0]);
+        else
+            k0 = v[0];
+#pragma unroll
+        for (int32_t i = 1; i < 4; i++)
+            v[i] = __viaddmax_s32(v[i - 1], gap, v[i]);
+        quad_store<ScoreT>(drow + j, s3, v[0], v[1], v[2]); // the first unit is rewritten in pass 2
+        s3 = v[3];
+#pragma unroll
+        for (int32_t i = 0; i < 4; i++)
+        {
+            b0[i] = n0[i];
+            if (TWO)
+                b1[i] = n1[i];
+        }
+        o0 += 4;
+        o1 += 4;
     }
+    // ---- carry: lane 0 starts from cin
+    int32_t L = __shfl_up_sync(kFull, s3, 1);
+    if (lane == 0)
+        L = cin;
+    if (__ballot_sync(kFull, L + gap > k0) != 0u)
+    {
+        // a horizontal run enters a strip from the left: max-plus prefix scan over the strip ends
+        const int32_t gl = S * gap;
+        int32_t v        = s3 - gl * (lane + 1);
+#pragma unroll
+        for (int32_t d = 1; d < 32; d <<= 1)
+        {
+            const int32_t o = __shfl_up_sync(kFull, v, d);
+            if (lane >= d)
+                v = max(v, o);
+        }
+        const int32_t excl = __shfl_up_sync(kFull, v, 1);
+        L                  = ((lane == 0) ? cin : max(cin, excl)) + gl * lane;
+    }
+    // ---- pass 2. Slot unit j holds the cells j - 1 .. j + 2 of the strip; while the last of them was improved, the next may be.
+    int32_t y[4];
+    quad_load<ScoreT>(drow, y);
+    bool more = L + 3 * gap > y[3];
+    quad_store<ScoreT>(drow, (lane == 0) ? local0 : L, max(y[1], L + gap), max(y[2], L + 2 * gap), max(y[3], L + 3 * gap));
+    for (int32_t j = 4; more && j < S; j += 4)
+    {
+        quad_load<ScoreT>(drow + j, y);
+        more = L + (j + 3) * gap > y[3];
+        quad_store<ScoreT>(drow + j, max(y[0], L + j * gap), max(y[1], L + (j + 1) * gap), max(y[2], L + (j + 2) * gap),
+                           max(y[3], L + (j + 3) * gap));
+    }
+    return max(s3, L + S * gap);
 }
 
 // The DP rows of needlemanWunschBanded (cudapoa_nw_banded.cuh:266-405) for one warp; everything before and after them (band
@@ -356,10 +448,9 @@ __device__ __forceinline__ void row_group_v3(const RowCtx<ScoreT>& cx, const int
 template <typename ScoreT, typename SizeT>
 __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const uint8_t* __restrict__ read, const Band<ScoreT>& B,
                            const int32_t band_width, const int32_t max_column, const int32_t gap, const int32_t mismatch, const int32_t match,
-                           int4* row_meta, uint8_t* pool, const int32_t pool_bytes, int4* srec, const int32_t max_group32)
+                           int4* row_meta, uint8_t* pool, const int32_t pool_bytes, int4* srec)
 {
     constexpr int32_t kMin   = min_score_of<ScoreT>();
-    const int32_t max_group  = sizeof(ScoreT) == 2 ? 2 : max_group32; // chunks per straight-line group of a fast row
     const int32_t lane       = threadIdx.x & 31;
     const int32_t stride     = B.stride;
     ScoreT* const scores     = B.scores;
@@ -371,6 +462,13 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
     const int32_t R          = min(pool_bytes / rowbytes, 64);
     if (R < 2)
         __trap(); // guard: v3_pool_bytes never launches a pool this small
+    // Fast rows run as strips of S cells per lane (strip_row_v3) when the band is wider than one chunk of 256 columns and a multiple
+    // of 128 (BatchConfig rounds it up; a hand-filled config need not), and a strip is not a multiple of 128 bytes. Otherwise they
+    // run in chunks (row_chunk_v3): a band of one chunk already needs one carry per row, and with strips of 128 bytes (int32 at
+    // band 1024) the 8 lanes of a shared-memory phase address the same banks in every unit (those rows ran 40 % slower than in
+    // chunks on an H100).
+    const int32_t S          = band_width / 32;
+    const bool strips        = band_width > kChunk && (band_width & 127) == 0 && (S * static_cast<int32_t>(sizeof(ScoreT))) % 128 != 0;
 
     // row 0: scores[j] = j * gap (:269-272), also into ring slot 0
     for (int32_t j = lane; j < stride; j += 32)
@@ -507,44 +605,44 @@ __device__ void dp_rows_v3(const Win<SizeT>& g, const int32_t graph_count, const
                 }
                 local0 = (bs == 0) ? (pc == 0 ? gap : first) : kMin;
                 cin    = (pc == 0) ? 0 : first;
-                int32_t cleft = local0;
-                // Chunks are taken in groups of up to max_group (row_group_v3): the candidate values and the lane-local closure
-                // of the chunks of a group are independent of each other, so their loads and arithmetic overlap; only the carry
-                // between chunks is sequential, and in the common case it is a scalar chain over values that are already known.
-                RowCtx<ScoreT> cx;
-                cx.prow0 = prow0;
-                cx.prow1 = prow1;
-                cx.rd    = read + bs;
-                cx.drow  = srow;
-                cx.sh0   = sh0;
-                cx.lim0  = lim0;
-                cx.sh1   = sh1;
-                cx.lim1  = lim1;
-                cx.base  = base;
-                cx.base4 = static_cast<uint32_t>(base) * 0x01010101u;
-                cx.bw    = band_width;
-                cx.gap   = gap;
-                cx.match = match;
-                cx.mismatch = mismatch;
-                // Few, compact instantiations run as loops: what the row loop executes has to stay resident in the instruction
-                // caches with many windows per SM at different places of it (a fully unrolled 8-variant version stalls on
-                // instruction fetch)
-                int32_t c0 = 0;
-                if (pc == 2)
+                const uint32_t base4 = static_cast<uint32_t>(base) * 0x01010101u;
+                if (strips)
                 {
-                    if (max_group >= 2)
-                        for (; c0 + 2 <= nchunks; c0 += 2)
-                            row_group_v3<ScoreT, 2, true>(cx, c0, lane, cin, cleft);
-                    for (; c0 < nchunks; c0++)
-                        row_group_v3<ScoreT, 1, true>(cx, c0, lane, cin, cleft);
+                    const int32_t c0 = S * lane;
+                    int32_t last;
+                    if (pc == 2)
+                        last = strip_row_v3<ScoreT, true>(prow0, sh0 + c0, lim0, prow1, sh1 + c0, lim1, read + bs + c0, base4, srow + c0, S,
+                                                          cin, local0, gap, match, mismatch, lane);
+                    else
+                        last = strip_row_v3<ScoreT, false>(prow0, sh0 + c0, lim0, prow1, sh1 + c0, lim1, read + bs + c0, base4, srow + c0, S,
+                                                           cin, local0, gap, match, mismatch, lane);
+                    cin = __shfl_sync(kFull, last, 31);
                 }
                 else
                 {
-                    if (max_group >= 2)
-                        for (; c0 + 2 <= nchunks; c0 += 2)
-                            row_group_v3<ScoreT, 2, false>(cx, c0, lane, cin, cleft);
-                    for (; c0 < nchunks; c0++)
-                        row_group_v3<ScoreT, 1, false>(cx, c0, lane, cin, cleft);
+                    RowCtx<ScoreT> cx;
+                    cx.prow0    = prow0;
+                    cx.prow1    = prow1;
+                    cx.rd       = read + bs;
+                    cx.drow     = srow;
+                    cx.sh0      = sh0;
+                    cx.lim0     = lim0;
+                    cx.sh1      = sh1;
+                    cx.lim1     = lim1;
+                    cx.base     = base;
+                    cx.base4    = base4;
+                    cx.bw       = band_width;
+                    cx.gap      = gap;
+                    cx.match    = match;
+                    cx.mismatch = mismatch;
+                    int32_t cleft = local0;
+                    for (int32_t c = 0; c < nchunks; c++)
+                    {
+                        if (pc == 2)
+                            row_chunk_v3<ScoreT, true>(cx, c, lane, cin, cleft);
+                        else
+                            row_chunk_v3<ScoreT, false>(cx, c, lane, cin, cleft);
+                    }
                 }
             }
             else
@@ -1599,7 +1697,7 @@ template <typename ScoreT, typename SizeT>
 __device__ int32_t nw_banded_v3(const Win<SizeT>& g, int32_t graph_count, const uint8_t* read, int32_t read_length, ScoreT* scores,
                                 float max_buffer_size, SizeT* aln_graph, SizeT* aln_read, int32_t band_width, int32_t gap, int32_t mismatch,
                                 int32_t match, int32_t rerun, const bool Adaptive, unsigned long long& cells, int4* row_meta, uint8_t* pool,
-                                int32_t pool_bytes, unsigned long long* timers, V3Shared* sh, const int32_t max_group32)
+                                int32_t pool_bytes, unsigned long long* timers, V3Shared* sh)
 {
     GWB200_TIMER_START();
     const float gradient     = __fdividef(static_cast<float>(read_length + 1), static_cast<float>(graph_count + 1));
@@ -1641,8 +1739,7 @@ __device__ int32_t nw_banded_v3(const Win<SizeT>& g, int32_t graph_count, const 
         cells += static_cast<unsigned long long>(graph_count) * static_cast<unsigned long long>(band_width);
 
     Band<ScoreT> B{scores, band_width, band_shift, max_column, band_width + kRightPad, gradient};
-    dp_rows_v3<ScoreT, SizeT>(g, graph_count, read, B, band_width, max_column, gap, mismatch, match, row_meta, pool, pool_bytes, sh->rec[0],
-                              max_group32);
+    dp_rows_v3<ScoreT, SizeT>(g, graph_count, read, B, band_width, max_column, gap, mismatch, match, row_meta, pool, pool_bytes, sh->rec[0]);
     GWB200_TIMER_LAP(0);
     int32_t result;
     if (pool_bytes >= TileBuf<ScoreT>::kBytes * 2)
@@ -1764,7 +1861,7 @@ __device__ void process_window_v3(const DeviceParams& P, const V2Extra& X, const
                 {
                     alen = nw_banded_v3<ScoreT, SizeT>(g, node_count, sequence, seq_len, scores, banded_buffer_size, aln_graph, aln_read,
                                                        P.band_width, P.gap, P.mismatch, P.match, rerun, adaptive, cells, row_meta, pool,
-                                                       X.pool_bytes, timers, sh, Y.max_group32);
+                                                       X.pool_bytes, timers, sh);
                     if (!adaptive || attempt == 1 || !(alen == kShiftLeft || alen == kShiftRight))
                         break;
                     rerun = alen; // rerun with extended and shifted band (cudapoa_kernels.cuh:374-396)
