@@ -2,13 +2,11 @@
 //
 // Host-side behaviour follows cudapoa/src/cudapoa_batch.cuh (admission, packing, status decoding) and
 // cudapoa/src/batch.cu (BatchConfig derivation, type selection via cudapoa_limits.hpp); memory layout and kernels are
-// this repo's own (poa_kernels.cuh). There is no CPU fallback: every entry needs a CUDA device.
+// this repo's own (poa_window_kernels.cuh). There is no CPU fallback: every entry needs a CUDA device.
 
 #include "../../include/gwb200.h"
 #include "common.cuh"
-#include "poa_kernels.cuh"
-#include "poa_kernels_tb.cuh"
-#include "poa_kernels_v3.cuh"
+#include "poa_window_kernels.cuh"
 
 #include <atomic>
 #include <cstdlib>
@@ -122,7 +120,6 @@ struct gwb200_poa_batch
     bool owns_dblock = true; // false: the block belongs to the caller's allocator (create_batch overload with an allocator)
     DeviceParams P{};
     V2Extra X{};
-    V3Extra Y{};
     PoaKernel kernel = PoaKernel::v3;
     bool tb_mode = false;    // static_band_traceback / adaptive_band_traceback
     int32_t trace_bytes = 2; // sizeof(TraceT): 1 unless max_banded_pred_distance > 127 (cudapoa_limits.hpp:56-60)
@@ -243,15 +240,21 @@ int32_t tb_pool_bytes(const gwb200_poa_batch* b)
     return static_cast<int32_t>(std::max<int64_t>(dflt, align_up64(need, 1024)));
 }
 
+// Dynamic shared memory per CTA of the first-generation kernel, where only the topological sort uses it (a 528-byte FIFO window plus
+// in-degree counters; the counters of further nodes stay in global memory). Its DP rows read the rows before them from global memory
+// through L1, so it leaves the shared-memory carve-out to the driver, which takes the smallest one that gives full residency: with
+// the largest carve-out (28 KB of L1 left) it ran 10-15 % slower at static band 2048 on an H100.
+constexpr int32_t kV1PoolBytes = 1024;
+
 // Resident CTAs per SM of a one-warp kernel with `smem` bytes of dynamic shared memory, after making that pool size launchable.
-// The kernel's residency is sized against the full shared-memory carve-out; do not inherit a device-wide cache preference
-// another library set in this process (the reference does cudaDeviceSetCacheConfig(PreferL1), cudapoa_kernels.cuh:605).
+// The kernel's residency is sized against the carve-out asked for here (the full one unless the caller needs less shared memory);
+// do not inherit a device-wide cache preference another library set in this process (the reference does cudaDeviceSetCacheConfig(PreferL1), cudapoa_kernels.cuh:605).
 template <typename Kernel>
-int32_t pooled_occupancy(Kernel kfn, int32_t smem)
+int32_t pooled_occupancy(Kernel kfn, int32_t smem, int32_t carveout = cudaSharedmemCarveoutMaxShared)
 {
     if (smem > 48 * 1024)
         cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    cudaFuncSetAttribute(kfn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(kfn, cudaFuncAttributePreferredSharedMemoryCarveout, carveout);
     int nb = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kfn, 32, smem) != cudaSuccess)
     {
@@ -265,47 +268,27 @@ int32_t pooled_occupancy(Kernel kfn, int32_t smem)
 template <typename ScoreT, typename SizeT>
 int32_t typed_action(gwb200_poa_batch* b, int action)
 {
-    if (b->kernel == PoaKernel::v1)
-    {
-        if (action == 1)
-        {
-            int nb = 0;
-            auto kfn = poa_window_kernel<ScoreT, SizeT, false>;
-            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kfn, 32, 0) != cudaSuccess)
-            {
-                cudaGetLastError();
-                return 0;
-            }
-            return nb;
-        }
-        dim3 grid(b->poa_count), block(32);
-        if (b->msa)
-            poa_window_kernel<ScoreT, SizeT, true><<<grid, block, 0, b->stream>>>(b->P);
-        else
-            poa_window_kernel<ScoreT, SizeT, false><<<grid, block, 0, b->stream>>>(b->P);
-        count_launch();
-        return 0;
-    }
-    const bool v3      = b->kernel == PoaKernel::v3;
+    void (*kfn)(const DeviceParams, const V2Extra) = poa_window_kernel<ScoreT, SizeT>;
+    if (b->kernel == PoaKernel::v3)
+        kfn = poa_window_kernel_v3<ScoreT, SizeT>;
+    else if (b->kernel == PoaKernel::tb)
+        kfn = poa_window_kernel_tb<ScoreT, SizeT>;
     const int32_t smem = b->X.pool_bytes;
-    const int32_t nb   = v3 ? pooled_occupancy(poa_window_kernel_v3<ScoreT, SizeT>, smem) : pooled_occupancy(poa_window_kernel_tb<ScoreT, SizeT>, smem);
+    const int32_t nb   = b->kernel == PoaKernel::v1 ? pooled_occupancy(kfn, smem, cudaSharedmemCarveoutDefault) : pooled_occupancy(kfn, smem);
     if (action == 1)
         return nb;
     b->X.timers = b->timers_on ? b->d_timers : nullptr;
     if (b->timers_on)
         cudaMemsetAsync(b->d_timers, 0, sizeof(unsigned long long) * 8 * b->poa_count, b->stream);
-    if (v3)
+    int32_t grid = b->poa_count;
+    if (b->kernel == PoaKernel::v3)
     {
         int sms = 132;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, b->device_id);
-        const int32_t grid = std::max(1, std::min(b->poa_count, std::max(1, nb) * sms));
-        cudaMemsetAsync(b->Y.work_counter, 0, sizeof(int32_t), b->stream);
-        poa_window_kernel_v3<ScoreT, SizeT><<<grid, 32, smem, b->stream>>>(b->P, b->X, b->Y);
+        grid = std::max(1, std::min(b->poa_count, std::max(1, nb) * sms));
+        cudaMemsetAsync(b->X.work_counter, 0, sizeof(int32_t), b->stream);
     }
-    else
-    {
-        poa_window_kernel_tb<ScoreT, SizeT><<<b->poa_count, 32, smem, b->stream>>>(b->P, b->X);
-    }
+    kfn<<<grid, 32, smem, b->stream>>>(b->P, b->X);
     count_launch();
     return 0;
 }
@@ -697,7 +680,7 @@ static int poa_batch_create_impl(gwb200_poa_batch** out, int32_t device_id, void
         b->X.rd_capacity = align_up(std::max(cfg->max_sequence_size, 1), 4) + 8;
         b->X.rd_node     = dc.take<uint8_t>(n * static_cast<int64_t>(b->X.rd_capacity) * S);
         b->d_timers      = dc.take<unsigned long long>(n * 8);
-        b->Y.work_counter = dc.take<int32_t>(64);
+        b->X.work_counter = dc.take<int32_t>(64);
         b->X.timers      = nullptr;
         b->X.tb_scores   = nullptr;
         b->X.tb_trace    = nullptr;
@@ -735,6 +718,8 @@ static int poa_batch_create_impl(gwb200_poa_batch** out, int32_t device_id, void
         b->X.pool_bytes = v3_pool_bytes(b);
     else if (b->kernel == PoaKernel::tb)
         b->X.pool_bytes = tb_pool_bytes(b);
+    else
+        b->X.pool_bytes = kV1PoolBytes;
     gwb200_poa_batch_reset(b);
     *out = b;
     return 0;
@@ -969,7 +954,7 @@ int32_t gwb200_poa_batch_kernel(const gwb200_poa_batch* b)
         return -1;
     return b->kernel == PoaKernel::tb ? 0 : (b->kernel == PoaKernel::v3 ? 1 : 2);
 }
-int32_t gwb200_poa_batch_pool_bytes(const gwb200_poa_batch* b) { return (b && b->kernel != PoaKernel::v1) ? b->X.pool_bytes : 0; }
+int32_t gwb200_poa_batch_pool_bytes(const gwb200_poa_batch* b) { return b ? b->X.pool_bytes : 0; }
 
 int gwb200_poa_batch_upload(gwb200_poa_batch* b)
 {

@@ -1,4 +1,5 @@
-// gw-b200 POA device code (sm_90a). One POA window per CTA.
+// gw-b200 POA device code (sm_90a): the batch layout, the first-generation alignments (nw_banded, nw_full), racon's sort and the
+// consensus / MSA generation that every window kernel (poa_window_kernels.cuh) shares.
 //
 // Behavioural contract = the reference's generatePOAKernel + generateConsensusKernel / generateMSAKernel
 // (cudapoa/src/cudapoa_kernels.cuh:76-542, cudapoa_nw_banded.cuh:177-557, cudapoa_nw.cuh:149-454,
@@ -718,155 +719,6 @@ __device__ int32_t nw_full(const Win<SizeT>& g, int32_t graph_count, const uint8
     return aligned_nodes;
 }
 
-// addAlignmentToGraph, cudapoa_add_alignment.cuh:65-285 (single thread). `path` (MSA only) records the node id of every
-// read base; it replaces the reference's per-edge read lists (outgoing_edges_coverage) with identical MSA output.
-template <typename SizeT, bool MSA>
-__device__ uint8_t add_alignment(const Win<SizeT>& g, int32_t& node_count_io, int32_t alignment_length, const SizeT* aln_graph,
-                                 const uint8_t* read, const SizeT* aln_read, const int8_t* base_weights, SizeT* path)
-{
-    int32_t node_count   = node_count_io;
-    int32_t head_node_id = -1;
-    int32_t curr_node_id = -1;
-    uint16_t prev_weight = 0;
-    const uint32_t limit = static_cast<uint32_t>(g.max_nodes);
-    for (int32_t pos = alignment_length - 1; pos >= 0; pos--)
-    {
-        const int32_t read_pos = aln_read[pos];
-        if (read_pos == -1)
-            continue;
-        const int8_t node_weight    = base_weights[read_pos];
-        const uint8_t read_base     = read[read_pos];
-        const int32_t graph_node_id = aln_graph[pos];
-        if (graph_node_id == -1)
-        {
-            curr_node_id = node_count++;
-            if (static_cast<uint32_t>(node_count) >= limit)
-                return static_cast<uint8_t>(st_node_count_exceeded_maximum_graph_size);
-            g.nodes[curr_node_id]   = read_base;
-            g.out_cnt[curr_node_id] = 0;
-            g.in_cnt[curr_node_id]  = 0;
-            g.aln_cnt[curr_node_id] = 0;
-            g.cov[curr_node_id]     = 0;
-        }
-        else
-        {
-            const uint8_t graph_base = g.nodes[graph_node_id];
-            if (graph_base == read_base)
-            {
-                curr_node_id = graph_node_id;
-            }
-            else
-            {
-                const int32_t num_aligned = g.aln_cnt[graph_node_id];
-                int32_t aligned_node_id   = -1;
-                for (int32_t n = 0; n < num_aligned; n++)
-                {
-                    const int32_t aid = g.aln(graph_node_id, n);
-                    if (g.nodes[aid] == read_base)
-                    {
-                        aligned_node_id = aid;
-                        break;
-                    }
-                }
-                if (aligned_node_id != -1)
-                {
-                    curr_node_id = aligned_node_id;
-                }
-                else
-                {
-                    curr_node_id = node_count++;
-                    if (static_cast<uint32_t>(node_count) >= limit)
-                        return static_cast<uint8_t>(st_node_count_exceeded_maximum_graph_size);
-                    g.nodes[curr_node_id]   = read_base;
-                    g.out_cnt[curr_node_id] = 0;
-                    g.in_cnt[curr_node_id]  = 0;
-                    g.cov[curr_node_id]     = 0;
-                    int32_t new_alignments  = 0;
-                    for (int32_t n = 0; n < num_aligned; n++)
-                    {
-                        const int32_t aid       = g.aln(graph_node_id, n);
-                        const int32_t aid_count = g.aln_cnt[aid];
-                        g.aln(aid, aid_count)   = static_cast<SizeT>(curr_node_id);
-                        g.aln_cnt[aid]          = static_cast<uint16_t>(aid_count + 1);
-                        g.aln(curr_node_id, new_alignments) = static_cast<SizeT>(aid);
-                        new_alignments++;
-                    }
-                    g.aln(graph_node_id, num_aligned) = static_cast<SizeT>(curr_node_id);
-                    g.aln_cnt[graph_node_id]          = static_cast<uint16_t>(num_aligned + 1);
-                    g.aln(curr_node_id, new_alignments) = static_cast<SizeT>(graph_node_id);
-                    new_alignments++;
-                    g.aln_cnt[curr_node_id] = static_cast<uint16_t>(new_alignments);
-                }
-            }
-        }
-        if (MSA)
-            path[read_pos] = static_cast<SizeT>(curr_node_id);
-
-        if (head_node_id != -1)
-        {
-            bool edge_exists       = false;
-            const int32_t in_count = g.in_cnt[curr_node_id];
-            for (int32_t e = 0; e < in_count; e++)
-            {
-                if (g.in_edge(curr_node_id, e) == head_node_id)
-                {
-                    edge_exists = true;
-                    g.w(curr_node_id, e) = static_cast<uint16_t>(g.w(curr_node_id, e) + (prev_weight + node_weight));
-                }
-            }
-            if (!edge_exists)
-            {
-                g.in_edge(curr_node_id, in_count) = static_cast<SizeT>(head_node_id);
-                g.w(curr_node_id, in_count)       = static_cast<uint16_t>(prev_weight + node_weight);
-                g.in_cnt[curr_node_id]            = static_cast<uint16_t>(in_count + 1);
-                const int32_t out_count           = g.out_cnt[head_node_id];
-                g.out_edge(head_node_id, out_count) = static_cast<SizeT>(curr_node_id);
-                g.out_cnt[head_node_id]             = static_cast<uint16_t>(out_count + 1);
-                if (out_count + 1 >= kMaxEdges || in_count + 1 >= kMaxEdges)
-                    return static_cast<uint8_t>(st_edge_count_exceeded_maximum_graph_size);
-            }
-        }
-        head_node_id = curr_node_id;
-        g.cov[head_node_id]++;
-        prev_weight = static_cast<uint16_t>(node_weight);
-    }
-    node_count_io = node_count;
-    return 0;
-}
-
-// topologicalSortDeviceUtil, cudapoa_topsort.cuh:45-97 (single thread)
-template <typename SizeT>
-__device__ void topsort(const Win<SizeT>& g, int32_t node_count)
-{
-    int32_t p = 0;
-    for (int32_t n = 0; n < node_count; n++)
-    {
-        const uint16_t c = g.in_cnt[n];
-        g.local_cnt[n]   = c;
-        if (c == 0)
-        {
-            g.pos[n]      = static_cast<SizeT>(p);
-            g.sorted[p++] = static_cast<SizeT>(n);
-        }
-    }
-    for (int32_t n = 0; n < p; n++)
-    {
-        const int32_t node = g.sorted[n];
-        const int32_t oc   = g.out_cnt[node];
-        for (int32_t e = 0; e < oc; e++)
-        {
-            const int32_t out_node = g.out_edge(node, e);
-            uint16_t c             = g.local_cnt[out_node];
-            if (--c == 0)
-            {
-                g.pos[out_node] = static_cast<SizeT>(p);
-                g.sorted[p++]   = static_cast<SizeT>(out_node);
-            }
-            g.local_cnt[out_node] = c;
-        }
-    }
-}
-
 // raconTopologicalSortDeviceUtil, cudapoa_topsort.cuh:103-197 (single thread)
 template <typename SizeT>
 __device__ bool racon_topsort(const Win<SizeT>& g, int32_t node_count, uint8_t* marks, uint8_t* check, SizeT* stack, int32_t stack_capacity)
@@ -1158,205 +1010,6 @@ __device__ int32_t generate_msa(const Win<SizeT>& g, int32_t node_count, int32_t
         off += (len + 3) & ~3;
     }
     return 0;
-}
-
-// The whole per-window pipeline. One warp per window (CTA = 32 threads), grid = n_windows.
-template <typename ScoreT, typename SizeT, bool MSA>
-__global__ void __launch_bounds__(32, 16) poa_window_kernel(const DeviceParams P)
-{
-    const int32_t w    = blockIdx.x;
-    const int32_t lane = threadIdx.x & 31;
-    if (w >= P.n_windows)
-        return;
-    const WindowInfo wi = P.windows[w];
-    const int64_t mn    = P.max_nodes;
-
-    Win<SizeT> g;
-    g.max_nodes = P.max_nodes;
-    g.nodes     = P.nodes + w * mn;
-    g.in_cnt    = P.in_cnt + w * mn;
-    g.out_cnt   = P.out_cnt + w * mn;
-    g.aln_cnt   = P.aln_cnt + w * mn;
-    g.cov       = P.node_cov + w * mn;
-    g.local_cnt = P.local_cnt + w * mn;
-    g.in_edges  = static_cast<SizeT*>(P.in_edges) + w * mn * kMaxEdges;
-    g.out_edges = static_cast<SizeT*>(P.out_edges) + w * mn * kMaxEdges;
-    g.aligned   = static_cast<SizeT*>(P.aligned) + w * mn * kMaxAligned;
-    g.in_w      = P.in_w + w * mn * kMaxEdges;
-    g.sorted    = static_cast<SizeT*>(P.sorted) + w * mn;
-    g.pos       = static_cast<SizeT*>(P.pos) + w * mn;
-
-    SizeT* aln_graph = static_cast<SizeT*>(P.aln_graph) + static_cast<int64_t>(w) * P.aln_capacity;
-    SizeT* aln_read  = static_cast<SizeT*>(P.aln_read) + static_cast<int64_t>(w) * P.aln_capacity;
-
-    const int32_t* seq_lengths = P.seq_lengths + wi.seq_len_offset;
-    const uint8_t* sequence    = P.sequences + wi.seq_start;
-    const int8_t* base_weights = P.weights + wi.seq_start;
-    SizeT* path                = MSA ? static_cast<SizeT*>(P.seq_path) + wi.seq_start : nullptr;
-
-    ScoreT* scores;
-    float banded_buffer_size = static_cast<float>(P.max_nodes) * static_cast<float>(P.matrix_seq_dim);
-    if (P.band_mode == bm_full_band)
-        scores = static_cast<ScoreT*>(P.scores) + wi.scores_offset * mn;
-    else
-        scores = static_cast<ScoreT*>(P.scores) + static_cast<int64_t>(banded_buffer_size) * static_cast<int64_t>(w);
-
-    uint8_t* consensus = P.consensus + static_cast<int64_t>(w) * P.max_consensus;
-    uint16_t* coverage = P.coverage + static_cast<int64_t>(w) * P.max_consensus;
-
-    // a group whose reads were all rejected stays in the batch with no read (add_poa_group returns empty_poa_group,
-    // cudapoa_batch.cuh:139-148): nothing to align, and seq_lengths[0] would belong to another window
-    if (wi.num_seqs <= 0)
-    {
-        if (threadIdx.x == 0)
-        {
-            consensus[0]       = 0;
-            P.status[w]        = st_empty_poa_group;
-            P.consensus_len[w] = 0;
-            P.node_count[w]    = 0;
-            P.cells[w]         = 0;
-        }
-        return;
-    }
-    // backbone from read 0, cudapoa_kernels.cuh:200-238 (lane-parallel here)
-    int32_t node_count = seq_lengths[0];
-    for (int32_t n = lane; n < node_count; n += 32)
-    {
-        g.nodes[n]   = sequence[n];
-        g.sorted[n]  = static_cast<SizeT>(n);
-        g.pos[n]     = static_cast<SizeT>(n);
-        g.aln_cnt[n] = 0;
-        g.cov[n]     = 1;
-        if (n > 0)
-        {
-            g.in_edge(n, 0)      = static_cast<SizeT>(n - 1);
-            g.w(n, 0)            = static_cast<uint16_t>(base_weights[n - 1] + base_weights[n]);
-            g.in_cnt[n]          = 1;
-            g.out_edge(n - 1, 0) = static_cast<SizeT>(n);
-            g.out_cnt[n - 1]     = 1;
-        }
-        else
-        {
-            g.in_cnt[0] = 0;
-            g.w(0, 0)   = static_cast<uint16_t>(base_weights[0]);
-        }
-        if (n == node_count - 1)
-            g.out_cnt[n] = 0;
-        if (MSA)
-            path[n] = static_cast<SizeT>(n);
-    }
-    __syncwarp();
-
-    unsigned long long cells = 0;
-    int32_t error            = 0;
-    const int32_t num_seqs   = wi.num_seqs;
-
-    for (int32_t s = 1; s < num_seqs; s++)
-    {
-        const int32_t seq_len = seq_lengths[s];
-        const int32_t adv     = (seq_lengths[s - 1] + 3) & ~3; // reads are padded to 4 bytes, cudapoa_batch.cuh:537
-        // NB: seq_lengths[0] is NOT overwritten with the node count here (the reference reuses that slot)
-        sequence += adv;
-        base_weights += adv;
-        if (MSA)
-            path += adv;
-
-        if (node_count >= P.max_nodes)
-        {
-            error = st_node_count_exceeded_maximum_graph_size;
-            break;
-        }
-        int32_t alen;
-        if (P.band_mode == bm_adaptive_band && P.band_width < kMaxAdaptiveBW)
-        {
-            alen = nw_banded<ScoreT, SizeT, true>(g, node_count, sequence, seq_len, scores, banded_buffer_size, aln_graph, aln_read, P.band_width,
-                                                  P.gap, P.mismatch, P.match, 0, cells);
-            __syncwarp();
-            if (alen == kShiftLeft || alen == kShiftRight)
-            {
-                alen = nw_banded<ScoreT, SizeT, true>(g, node_count, sequence, seq_len, scores, banded_buffer_size, aln_graph, aln_read,
-                                                      P.band_width, P.gap, P.mismatch, P.match, alen, cells);
-                __syncwarp();
-            }
-        }
-        else if (P.band_mode == bm_static_band || P.band_mode == bm_adaptive_band)
-        {
-            alen = nw_banded<ScoreT, SizeT, false>(g, node_count, sequence, seq_len, scores, banded_buffer_size, aln_graph, aln_read, P.band_width,
-                                                   P.gap, P.mismatch, P.match, 0, cells);
-            __syncwarp();
-        }
-        else
-        {
-            alen = nw_full<ScoreT, SizeT>(g, node_count, sequence, seq_len, scores, wi.scores_width, aln_graph, aln_read, P.gap, P.mismatch,
-                                          P.match, cells);
-            __syncwarp();
-        }
-        if (alen == kNWBacktrackFail)
-        {
-            error = st_loop_count_exceeded_upper_bound;
-            break;
-        }
-        if (alen == kNWStorageFail)
-        {
-            error = st_exceeded_adaptive_banded_matrix_size;
-            break;
-        }
-        if (alen < 0)
-            alen = 0; // a second rerun code: the reference's addAlignmentToGraph loop does not execute
-
-        if (lane == 0)
-        {
-            int32_t nc = node_count;
-            uint8_t e  = add_alignment<SizeT, MSA>(g, nc, alen, aln_graph, sequence, aln_read, base_weights, path);
-            if (e != 0)
-            {
-                error = e;
-            }
-            else
-            {
-                node_count = nc;
-                if (P.accurate)
-                    racon_topsort(g, node_count, P.marks + w * mn, P.check + w * mn,
-                                  static_cast<SizeT*>(P.stack) + static_cast<int64_t>(w) * P.stack_capacity, P.stack_capacity);
-                else
-                    topsort(g, node_count);
-            }
-        }
-        __syncwarp();
-        error      = __shfl_sync(kFull, error, 0);
-        node_count = __shfl_sync(kFull, node_count, 0);
-        if (error)
-            break;
-    }
-
-    int32_t cons_len = 0;
-    if (!error)
-    {
-        if (MSA)
-        {
-            error = generate_msa<SizeT>(g, node_count, num_seqs, seq_lengths, static_cast<SizeT*>(P.seq_path) + wi.seq_start,
-                                        static_cast<SizeT*>(P.msa_col) + w * mn, P.marks + w * mn, P.check + w * mn,
-                                        static_cast<SizeT*>(P.stack) + static_cast<int64_t>(w) * P.stack_capacity, P.stack_capacity,
-                                        P.msa_out + static_cast<int64_t>(w) * P.max_seqs * P.max_consensus, P.max_consensus);
-        }
-        else
-        {
-            error = generate_consensus<SizeT>(g, node_count, P.cons_scores + w * mn, static_cast<SizeT*>(P.cons_preds) + w * mn, consensus,
-                                              coverage, P.max_consensus, &cons_len);
-        }
-    }
-    if (lane == 0)
-    {
-        if (error)
-        {
-            consensus[0] = 0;
-            cons_len     = 0;
-        }
-        P.status[w]        = error;
-        P.consensus_len[w] = cons_len;
-        P.node_count[w]    = node_count;
-        P.cells[w]         = cells;
-    }
 }
 
 __global__ void fdividef_kernel(int32_t n, const float* a, const float* b, float* out)

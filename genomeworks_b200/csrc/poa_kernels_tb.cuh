@@ -398,202 +398,5 @@ __device__ int32_t nw_banded_tb(const Win<SizeT>& g, int32_t graph_count, const 
     return aligned_nodes;
 }
 
-// One window per CTA of one warp (cudapoa_kernels.cuh:200-541, alignment :270-346): nw_banded_tb, then the graph update and
-// topological sort that the v3 kernel also uses (poa_kernels_v2.cuh).
-template <typename ScoreT, typename SizeT>
-__global__ void __launch_bounds__(32, 16) poa_window_kernel_tb(const DeviceParams P, const V2Extra X)
-{
-    const bool MSA = P.msa != 0;
-    extern __shared__ __align__(16) uint8_t pool[];
-    const int32_t w    = blockIdx.x;
-    const int32_t lane = threadIdx.x & 31;
-    if (w >= P.n_windows)
-        return;
-    const WindowInfo wi = P.windows[w];
-    const int64_t mn    = P.max_nodes;
-    unsigned long long* timers = X.timers ? X.timers + static_cast<int64_t>(w) * 8 : nullptr;
-
-    Win<SizeT> g;
-    g.max_nodes = P.max_nodes;
-    g.nodes     = P.nodes + w * mn;
-    g.in_cnt    = P.in_cnt + w * mn;
-    g.out_cnt   = P.out_cnt + w * mn;
-    g.aln_cnt   = P.aln_cnt + w * mn;
-    g.cov       = P.node_cov + w * mn;
-    g.local_cnt = P.local_cnt + w * mn;
-    g.in_edges  = static_cast<SizeT*>(P.in_edges) + w * mn * kMaxEdges;
-    g.out_edges = static_cast<SizeT*>(P.out_edges) + w * mn * kMaxEdges;
-    g.aligned   = static_cast<SizeT*>(P.aligned) + w * mn * kMaxAligned;
-    g.in_w      = P.in_w + w * mn * kMaxEdges;
-    g.sorted    = static_cast<SizeT*>(P.sorted) + w * mn;
-    g.pos       = static_cast<SizeT*>(P.pos) + w * mn;
-
-    SizeT* aln_graph = static_cast<SizeT*>(P.aln_graph) + static_cast<int64_t>(w) * P.aln_capacity;
-    SizeT* aln_read  = static_cast<SizeT*>(P.aln_read) + static_cast<int64_t>(w) * P.aln_capacity;
-    SizeT* rd_node   = static_cast<SizeT*>(X.rd_node) + static_cast<int64_t>(w) * X.rd_capacity;
-
-    const int32_t* seq_lengths = P.seq_lengths + wi.seq_len_offset;
-    const uint8_t* sequence    = P.sequences + wi.seq_start;
-    const int8_t* base_weights = P.weights + wi.seq_start;
-    SizeT* path                = MSA ? static_cast<SizeT*>(P.seq_path) + wi.seq_start : nullptr;
-
-    // the score ring of this window, and its trace matrix in the pooled buffer
-    const float banded_buffer_size = static_cast<float>(P.max_nodes) * static_cast<float>(P.matrix_seq_dim);
-    ScoreT* tb_scores              = static_cast<ScoreT*>(X.tb_scores) + static_cast<int64_t>(w) * X.tb_height * P.matrix_seq_dim;
-    const int64_t toff             = static_cast<int64_t>(banded_buffer_size) * static_cast<int64_t>(w);
-
-    uint8_t* consensus = P.consensus + static_cast<int64_t>(w) * P.max_consensus;
-    uint16_t* coverage = P.coverage + static_cast<int64_t>(w) * P.max_consensus;
-
-    // a group whose reads were all rejected stays in the batch with no read (add_poa_group returns empty_poa_group,
-    // cudapoa_batch.cuh:139-148): nothing to align, and seq_lengths[0] would belong to another window
-    if (wi.num_seqs <= 0)
-    {
-        if (lane == 0)
-        {
-            consensus[0]       = 0;
-            P.status[w]        = st_empty_poa_group;
-            P.consensus_len[w] = 0;
-            P.node_count[w]    = 0;
-            P.cells[w]         = 0;
-        }
-        return;
-    }
-    // backbone from read 0 (cudapoa_kernels.cuh:200-238), lane-parallel
-    int32_t node_count = seq_lengths[0];
-    for (int32_t n = lane; n < node_count; n += 32)
-    {
-        g.nodes[n]   = sequence[n];
-        g.sorted[n]  = static_cast<SizeT>(n);
-        g.pos[n]     = static_cast<SizeT>(n);
-        g.aln_cnt[n] = 0;
-        g.cov[n]     = 1;
-        if (n > 0)
-        {
-            g.in_edge(n, 0)      = static_cast<SizeT>(n - 1);
-            g.w(n, 0)            = static_cast<uint16_t>(base_weights[n - 1] + base_weights[n]);
-            g.in_cnt[n]          = 1;
-            g.out_edge(n - 1, 0) = static_cast<SizeT>(n);
-            g.out_cnt[n - 1]     = 1;
-        }
-        else
-        {
-            g.in_cnt[0] = 0;
-            g.w(0, 0)   = static_cast<uint16_t>(base_weights[0]);
-        }
-        if (n == node_count - 1)
-            g.out_cnt[n] = 0;
-        if (MSA)
-            path[n] = static_cast<SizeT>(n);
-    }
-    __syncwarp();
-
-    unsigned long long cells = 0;
-    int32_t error            = 0;
-    const int32_t num_seqs   = wi.num_seqs;
-    const bool adaptive      = (P.band_mode == bm_adaptive_band_traceback && P.band_width < kMaxAdaptiveBW);
-
-    for (int32_t s = 1; s < num_seqs; s++)
-    {
-        const int32_t seq_len = seq_lengths[s];
-        const int32_t adv     = (seq_lengths[s - 1] + 3) & ~3;
-        sequence += adv;
-        base_weights += adv;
-        if (MSA)
-            path += adv;
-        if (node_count >= P.max_nodes)
-        {
-            error = st_node_count_exceeded_maximum_graph_size;
-            break;
-        }
-        int32_t alen;
-        int32_t rerun = 0;
-        for (int32_t attempt = 0; attempt < 2; attempt++)
-        {
-            if (X.tb_trace16)
-                alen = nw_banded_tb<ScoreT, SizeT, int16_t>(g, node_count, sequence, seq_len, tb_scores, static_cast<int16_t*>(X.tb_trace) + toff,
-                                                            banded_buffer_size, aln_graph, aln_read, P.band_width, X.tb_height, P.gap, P.mismatch,
-                                                            P.match, rerun, adaptive, cells);
-            else
-                alen = nw_banded_tb<ScoreT, SizeT, int8_t>(g, node_count, sequence, seq_len, tb_scores, static_cast<int8_t*>(X.tb_trace) + toff,
-                                                           banded_buffer_size, aln_graph, aln_read, P.band_width, X.tb_height, P.gap, P.mismatch,
-                                                           P.match, rerun, adaptive, cells);
-            if (!adaptive || attempt == 1 || !(alen == kShiftLeft || alen == kShiftRight))
-                break;
-            rerun = alen; // rerun with extended and shifted band (cudapoa_kernels.cuh:374-396)
-        }
-        if (alen == kNWTracebackBufferFail)
-        {
-            error = st_exceeded_maximum_predecessor_distance;
-            break;
-        }
-        if (alen == kNWBacktrackFail)
-        {
-            error = st_loop_count_exceeded_upper_bound;
-            break;
-        }
-        if (alen == kNWStorageFail)
-        {
-            error = st_exceeded_adaptive_banded_matrix_size;
-            break;
-        }
-        if (alen < 0)
-            alen = 0;
-        unsigned long long t_ph__ = timers ? clock64() : 0ull;
-        int32_t nc                = node_count;
-        error = add_alignment_v2<SizeT>(g, nc, alen, aln_graph, sequence, seq_len, aln_read, base_weights, path, rd_node);
-        GWB200_TIMER_LAP(3);
-        if (!error)
-        {
-            if (P.accurate)
-            {
-                if (lane == 0)
-                    racon_topsort(g, nc, P.marks + w * mn, P.check + w * mn, static_cast<SizeT*>(P.stack) + static_cast<int64_t>(w) * P.stack_capacity,
-                                  P.stack_capacity);
-                __syncwarp();
-            }
-            else
-            {
-                topsort_v2<SizeT>(g, nc, pool, X.pool_bytes, static_cast<SizeT*>(P.cons_preds) + w * mn);
-            }
-        }
-        GWB200_TIMER_LAP(4);
-        node_count = nc;
-        if (error)
-            break;
-    }
-
-    int32_t cons_len = 0;
-    if (!error)
-    {
-        unsigned long long t_ph__ = timers ? clock64() : 0ull;
-        if (MSA)
-        {
-            error = generate_msa<SizeT>(g, node_count, num_seqs, seq_lengths, static_cast<SizeT*>(P.seq_path) + wi.seq_start,
-                                        static_cast<SizeT*>(P.msa_col) + w * mn, P.marks + w * mn, P.check + w * mn,
-                                        static_cast<SizeT*>(P.stack) + static_cast<int64_t>(w) * P.stack_capacity, P.stack_capacity,
-                                        P.msa_out + static_cast<int64_t>(w) * P.max_seqs * P.max_consensus, P.max_consensus);
-        }
-        else
-        {
-            error = generate_consensus<SizeT>(g, node_count, P.cons_scores + w * mn, static_cast<SizeT*>(P.cons_preds) + w * mn, consensus,
-                                              coverage, P.max_consensus, &cons_len);
-        }
-        GWB200_TIMER_LAP(5);
-    }
-    if (lane == 0)
-    {
-        if (error)
-        {
-            consensus[0] = 0;
-            cons_len     = 0;
-        }
-        P.status[w]        = error;
-        P.consensus_len[w] = cons_len;
-        P.node_count[w]    = node_count;
-        P.cells[w]         = cells;
-    }
-}
-
 } // namespace poa
 } // namespace gwb200

@@ -1,16 +1,11 @@
-// gw-b200 POA device code (sm_90a): the one-warp phases that the v3 kernel (poa_kernels_v3.cuh) and the traceback-mode kernel
-// (poa_kernels_tb.cuh) share, with the same behavioural contract as poa_kernels.cuh (identical consensus / coverage / MSA /
-// status to the reference kernels).
+// gw-b200 POA device code (sm_90a): the graph update that every window kernel (poa_window_kernels.cuh) runs, with the same
+// behavioural contract as poa_kernels.cuh (identical consensus / coverage / MSA / status to the reference kernels).
 //
 //   add alignment lane-parallel over read bases (new-node ids by ballot prefix sum); conflict-free because a path
 //                visits every node, ring and edge at most once.
-//   topsort      same Kahn FIFO order (cudapoa_topsort.cuh:45-97): in-degree counters, a tagged window of the FIFO and as
-//                many "only child" words as fit live in shared memory; single-child chains are followed in a register.
 //
 // Also the per-batch kernel arguments (V2Extra), the phase timers and small score-row helpers.
 #pragma once
-#include <type_traits>
-
 #include "poa_kernels.cuh"
 
 namespace gwb200
@@ -23,7 +18,8 @@ constexpr int32_t kTileCols = 64;
 
 struct V2Extra
 {
-    int4* row_meta;     // [n_windows][max_nodes + 1] : {node, pred0 row, pred1 row, base | pc << 8 | sink << 16 | band_start / 4 << 17}
+    int4* row_meta;     // [n_windows][max_nodes + 1] : v3 rows {node, pred0 row, pred1 row, base | pc << 8 | sink << 16 | band_start / 4 << 17};
+                        // every kernel's topological sort uses it as scratch between alignments
     void* rd_node;      // SizeT [n_windows][max_seq_aligned] : graph node aligned to each read base (-1 = insertion)
     int32_t rd_capacity;
     int32_t pool_bytes; // dynamic shared memory per CTA
@@ -34,6 +30,7 @@ struct V2Extra
     int32_t tb_height;
     int32_t tb_trace16;
     unsigned long long* timers; // optional [n_windows][8] phase cycle counters (nullptr = off)
+    int32_t* work_counter;      // v3: next window index (persistent grid), reset by the host before every launch
 };
 
 #define GWB200_TIMER_START() unsigned long long t_ph__ = timers ? clock64() : 0ull
@@ -228,153 +225,6 @@ __device__ int32_t add_alignment_v2(const Win<SizeT>& g, int32_t& node_count_io,
     if (!error)
         node_count_io = node_count;
     return error;
-}
-
-// topologicalSortDeviceUtil (cudapoa_topsort.cuh:45-97): same Kahn FIFO order. The in-degree counters (u8) and a 64-entry
-// tagged window of the FIFO live in the shared-memory pool; a compressed "only child" word per node (SizeT wide) lives in the
-// pool too as far as it fits, the words of the remaining (highest) node ids in a global scratch array (chains run along
-// consecutive node ids, so those loads hit L1).
-// Both are filled by coalesced loads; the serial walk touches the adjacency arrays only at branching nodes and global memory
-// otherwise only to write sorted[] / pos[].
-template <typename SizeT, typename WordT>
-__device__ void topsort_walk(const Win<SizeT>& g, int32_t node_count, int32_t* q_tag, int32_t* q_node, uint8_t* cnt, WordT* e0s,
-                             int32_t n_shared, WordT* e0g)
-{
-    // child word of node n: e0s[n] (shared memory) for n < n_shared, e0g[n] (global scratch) otherwise
-    const int32_t lane     = threadIdx.x & 31;
-    constexpr int32_t kQ   = 64;
-    constexpr WordT kOne   = static_cast<WordT>(1) << (8 * sizeof(WordT) - 1); // flag: exactly one out edge
-    constexpr WordT kNone  = static_cast<WordT>(kOne - 1);                     // no out edge
-    // e0w[n]: kOne | child -> exactly one out edge;  kNone -> no out edge;  else first child of several (count and the other
-    // children come from global memory, both loads issued together)
-    for (int32_t k = lane; k < kQ; k += 32)
-        q_tag[k] = -1;
-    __syncwarp();
-    int32_t p = 0;
-    for (int32_t n0 = 0; n0 < node_count; n0 += 32)
-    {
-        const int32_t n = n0 + lane;
-        int32_t c       = 1;
-        if (n < node_count)
-        {
-            c                = g.in_cnt[n];
-            const int32_t oc = g.out_cnt[n];
-            const WordT e0   = static_cast<WordT>(static_cast<WordT>(g.out_edge(n, 0)) & kNone);
-            cnt[n]           = static_cast<uint8_t>(c);
-            const WordT wv   = static_cast<WordT>(oc == 0 ? kNone : (oc == 1 ? (kOne | e0) : e0));
-            if (n < n_shared)
-                e0s[n] = wv;
-            else
-                e0g[n] = wv;
-        }
-        const bool is_src = n < node_count && c == 0;
-        const uint32_t m  = __ballot_sync(kFull, is_src);
-        if (is_src)
-        {
-            const int32_t at = p + __popc(m & ((1u << lane) - 1));
-            g.pos[n]         = static_cast<SizeT>(at);
-            g.sorted[at]     = static_cast<SizeT>(n);
-            if (at < kQ)
-            {
-                q_node[at] = n;
-                q_tag[at]  = at;
-            }
-        }
-        p += __popc(m);
-    }
-    __syncwarp();
-    if (lane == 0)
-    {
-        int32_t n        = 0;
-        int32_t reg_node = -1; // node at position n when the FIFO held nothing else (chain following without the window)
-        while (n < p)
-        {
-            int32_t node = reg_node;
-            if (node < 0)
-            {
-                const int32_t slot = n & (kQ - 1);
-                node               = (q_tag[slot] == n) ? q_node[slot] : static_cast<int32_t>(g.sorted[n]);
-            }
-            reg_node      = -1;
-            const WordT w = node < n_shared ? e0s[node] : e0g[node];
-            n++;
-            if (w & kOne)
-            {
-                // exactly one child: the overwhelmingly common case in a POA graph
-                const int32_t child = static_cast<int32_t>(w & kNone);
-                const uint8_t c     = static_cast<uint8_t>(cnt[child] - 1);
-                cnt[child]          = c;
-                if (c == 0)
-                {
-                    g.pos[child] = static_cast<SizeT>(p);
-                    g.sorted[p]  = static_cast<SizeT>(child);
-                    if (p == n)
-                    {
-                        reg_node = child; // the FIFO was empty: the child is the next node to process
-                    }
-                    else if (p - kQ < n)
-                    {
-                        q_node[p & (kQ - 1)] = child;
-                        q_tag[p & (kQ - 1)]  = p;
-                    }
-                    p++;
-                }
-            }
-            else if (w != kNone)
-            {
-                const int32_t oc = g.out_cnt[node];
-                int32_t nxt      = g.out_edge(node, 1); // issued together with the count: one memory latency for the common 2-child node
-                int32_t child    = static_cast<int32_t>(w);
-                for (int32_t e = 0; e < oc; e++)
-                {
-                    if (e == 1)
-                        child = nxt;
-                    else if (e > 1)
-                        child = g.out_edge(node, e);
-                    const uint8_t c = static_cast<uint8_t>(cnt[child] - 1);
-                    cnt[child]      = c;
-                    if (c == 0)
-                    {
-                        g.pos[child] = static_cast<SizeT>(p);
-                        g.sorted[p]  = static_cast<SizeT>(child);
-                        if (p - kQ < n) // slot p % kQ held position p - kQ, already consumed
-                        {
-                            q_node[p & (kQ - 1)] = child;
-                            q_tag[p & (kQ - 1)]  = p;
-                        }
-                        p++;
-                    }
-                }
-            }
-        }
-    }
-    __syncwarp();
-}
-
-// `scratch`: a per-window global array of at least max_nodes SizeT-sized words that is free during the sort (cons_preds)
-template <typename SizeT>
-__device__ void topsort_v2(const Win<SizeT>& g, int32_t node_count, uint8_t* pool, int32_t pool_bytes, void* scratch)
-{
-    using WordT          = typename std::conditional<sizeof(SizeT) == 2, uint16_t, uint32_t>::type;
-    constexpr int32_t kQ = 64;
-    const int32_t nc4    = (node_count + 3) & ~3;
-    const int32_t fixed  = kQ * 8 + nc4 + 16;
-    int32_t* q_tag       = reinterpret_cast<int32_t*>(pool);
-    int32_t* q_node      = q_tag + kQ;
-    uint8_t* cnt         = pool + kQ * 8;
-    if (fixed <= pool_bytes)
-    {
-        // as many child words as fit stay in shared memory (low node ids: the first read's backbone), the rest go to `scratch`
-        const int32_t n_shared = min(node_count, (pool_bytes - fixed) / static_cast<int32_t>(sizeof(WordT)));
-        topsort_walk<SizeT, WordT>(g, node_count, q_tag, q_node, cnt, reinterpret_cast<WordT*>(pool + kQ * 8 + nc4), n_shared,
-                                   static_cast<WordT*>(scratch));
-    }
-    else
-    {
-        if ((threadIdx.x & 31) == 0)
-            topsort(g, node_count);
-        __syncwarp();
-    }
 }
 
 } // namespace poa

@@ -239,7 +239,7 @@ class CudaPoaBatch:
 
     @property
     def pool_bytes(self):
-        """Dynamic shared memory per CTA of the launch (0 for the first-generation kernel)."""
+        """Dynamic shared memory per CTA of the launch."""
         return lib().gwb200_poa_batch_pool_bytes(self._h)
 
     def last_cells(self):

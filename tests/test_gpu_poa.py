@@ -330,12 +330,13 @@ def test_c3_full_shape_msa_vs_reference():
 def test_empty_group_stays_in_the_batch_without_touching_other_windows():
     """A group whose reads are all rejected returns empty_poa_group but still occupies a slot (cudapoa_batch.cuh:139-148); the
     kernels must not read a read length for it (it would be the next window's). Its status is empty_poa_group, the windows
-    around it are unaffected."""
+    around it are unaffected. Runs on each of the three window kernels."""
     from genomeworks_b200 import cudapoa
-    cfg = cudapoa.make_config(1024, 10, 256, "static_band")
     good = ["ACGTTGCAAGCTTGCATGCA" * 10, "ACGTTGCAAGCTAGCATGCA" * 10, "ACGTTGCAAGCTTGCATGCA" * 10]
-    for kernel_env in (None,):
+    for kernel, band, mode in (("v3", 256, "static_band"), ("tb", 256, "static_band_traceback"), ("v1", 1664, "static_band")):
+        cfg = cudapoa.make_config(1024, 10, band, mode)
         b = cudapoa.CudaPoaBatch(10, 1024, 1 << 30, config=cfg)
+        assert cudapoa.KERNEL_NAMES[b.kernel] == kernel
         assert b.add_poa_group(good)[0] == cudapoa.success
         assert b.add_poa_group(["A" * 1025])[0] == cudapoa.empty_poa_group
         assert b.add_poa_group(good)[0] == cudapoa.success

@@ -386,11 +386,14 @@ def test_builders_edge_and_node_limits():
     assert int(r["status"][0]) == 5  # edge_count_exceeded_maximum_graph_size
     r = ol.poa_run([list(node_limit_window())], np.array((1024, 2048, 1100, 264, 256, 16, 1, 0), dtype=np.int32))
     assert int(r["status"][0]) == 4  # node_count_exceeded_maximum_graph_size
+    r = ol.poa_run([list(node_limit_window(1400, 200))], np.array((1664, 3328, 1664, 1672, 1664, 16, 1, 0), dtype=np.int32))
+    assert int(r["status"][0]) == 4
 
 
-def node_limit_window():
-    """Reads (at most 1024 bases) with long insertions: the graph passes 1100 nodes after a few reads."""
-    return build_window(44, 800, 10, long_ins=(100,) * 9, subs=0.05)
+def node_limit_window(backbone=800, insertion=100):
+    """Reads (at most backbone + insertion bases) with long insertions: the graph passes 1100 nodes (1664 with a backbone of 1400
+    and insertions of 200) after a few reads."""
+    return build_window(44, backbone, 10, long_ins=(insertion,) * 9, subs=0.05)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -482,6 +485,7 @@ def test_kernel_selection_band_1536_vs_1664(score, device_fdiv):
     ws = far_hub_windows(800, 1100, n=3, n_reads=6)
     run_and_check("static 1536 int%d (selection)" % score, ws, config(2048, 4096, 1536, "static_band"), 4 << 30, "v3", match=match)
     run_and_check("static 1664 int%d (selection)" % score, ws, config(2048, 4096, 1664, "static_band"), 4 << 30, "v1", match=match)
+    run_and_check("static 1664 int%d MSA (selection)" % score, ws, config(2048, 4096, 1664, "static_band"), 4 << 30, "v1", match=match, msa=True)
 
 
 @pytest.mark.gpu
@@ -517,14 +521,17 @@ def test_traceback_kernel_wide_bands(band, mode, score, device_fdiv):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("kernel", ["v3", "tb", "v1"])
 @pytest.mark.parametrize("mode", ["static_band", "adaptive_band"])
 @pytest.mark.parametrize("score", [16, 32])
-def test_v3_shape_and_status_edges(mode, score, device_fdiv):
+def test_shape_and_status_edges(kernel, mode, score, device_fdiv):
     """Windows of one read, reads of 1-5 and 31-33 bases and of exactly max_sequence_size, backbones of 31/32/33/64/65 bases
-    (either side of the 32-row record groups), N bases, a 51st edge and a graph that outgrows max_nodes, each between ordinary
-    windows of the same batch."""
+    (either side of v3's 32-row record groups), N bases, a 51st edge and a graph that outgrows max_nodes, each between ordinary
+    windows of the same batch, on each kernel: tb runs the traceback counterpart of the band mode, v1 a band of 1664 (which
+    needs reads and graphs of 1664)."""
     from genomeworks_b200 import cudapoa
     match = 8 if score == 16 else 40
+    max_seq, max_nodes, band = (1664, 1664, 1664) if kernel == "v1" else (1024, 1100, 256)
     rng = np.random.RandomState(900)
     plain = [build_window(910 + i, 500 + 37 * i, 5) for i in range(12)]
     edges = [(_rand(rng, 300),)]  # one read
@@ -534,18 +541,18 @@ def test_v3_shape_and_status_edges(mode, score, device_fdiv):
         edges.append(tuple([_rand(rng, n)] + [_substitute(rng, _rand(rng, n), 0) for _ in range(3)]))  # all reads short
     for n in (31, 32, 33, 64, 65):
         edges.append(build_window(930 + n, n, 6, subs=0.05))
-    edges.append(build_window(940, 1024, 4, subs=0.01))  # reads of exactly max_sequence_size (backbone) ...
-    edges[-1] = tuple(r[:1024] if len(r) > 1024 else r + "A" * (1024 - len(r)) for r in edges[-1])
+    edges.append(build_window(940, max_seq, 4, subs=0.01))  # reads of exactly max_sequence_size (backbone) ...
+    edges[-1] = tuple(r[:max_seq] if len(r) > max_seq else r + "A" * (max_seq - len(r)) for r in edges[-1])
     edges.append(build_window(941, 700, 6, ns=12))
     edges.append(build_window(942, 300, 6, ns=300, subs=0.0))
     edges.append(edge_limit_window())
     edges.append(wide_hub_window())
-    edges.append(node_limit_window())
+    edges.append(node_limit_window(1400, 200) if kernel == "v1" else node_limit_window())
     ws = []
     for i, e in enumerate(edges):
         ws += [e, plain[i % len(plain)]]
-    cfg = config(1024, 1100, 256, mode, nseq=128)
-    f = run_and_check("edges %s int%d" % (mode, score), ws, cfg, 8 << 30, "v3", match=match)
+    cfg = config(max_seq, max_nodes, band, mode + ("_traceback" if kernel == "tb" else ""), nseq=128, max_pred=2 * band)
+    f = run_and_check("edges %s %s int%d" % (kernel, mode, score), ws, cfg, 8 << 30, kernel, match=match)
     st = f["statuses"]
     assert cudapoa.edge_count_exceeded_maximum_graph_size in st and cudapoa.node_count_exceeded_maximum_graph_size in st
     assert all(s == 0 for s in st[1::2]), "a neighbouring window failed"

@@ -1,8 +1,9 @@
 """Where the POA kernel spends its time: C3 of bench.py (640 windows of 10 kb x 32 reads, seeds 1000 + i, adaptive band 256,
 int32 scores, adaptive_storage_factor 3.0) with the device phase timers, plus the kernel time of static bands 512 / 1024 / 1536
-with int16 and int32 scores.
+with int16 and int32 scores on v3, of static band 2048 on the first-generation kernel and of static_band_traceback 256 / 1536 on
+the traceback-mode kernel.
 
-usage: poa_phase_split.py [--reps N] [--no-static]
+usage: poa_phase_split.py [--reps N] [--no-static] [--no-c3]
 Prints the card, the C3 kernel time (timers off, best of N), each phase's share of the summed phase cycles (timers on), and the
 dp_rows cycles per executed DP cell. Kernel times are CUDA-event times of one launch of the whole batch."""
 import os
@@ -55,13 +56,13 @@ def c3():
     b.close()
 
 
-def static_band(band, score):
+def static_band(band, score, mode="static_band", kernel="v3"):
     # config of the static-band cases of test_gpu_poa_kernel_paths.py: match 8 keeps int16 scores, 40 needs int32
     match = 8 if score == 16 else 40
-    cfg = cudapoa.make_config_explicit(3072, 6144, 4096, band, 16, band + 8, "static_band")
+    cfg = cudapoa.make_config_explicit(3072, 6144, 4096, band, 16, band + 8, mode, 2 * band if "traceback" in mode else 0)
     free_b, _ = torch.cuda.mem_get_info()
     b = cudapoa.CudaPoaBatch(16, 3072, int(free_b * 0.9), config=cfg, match_score=match)
-    assert b.score_bytes * 8 == score and cudapoa.KERNEL_NAMES[b.kernel] == "v3"
+    assert b.score_bytes * 8 == score and cudapoa.KERNEL_NAMES[b.kernel] == kernel
     n = min(b.max_poas, 4 * max(b.resident_windows, 1))
     rc, added = b.add_poa_groups_flat(*synth.poa_windows(n, 2500, 16, 50, 25, 25, seed0=5000, max_read_len=3072))
     assert rc == 0 and added == n
@@ -70,16 +71,21 @@ def static_band(band, score):
     b.launch()
     b.sync()
     ms = kernel_ms(b, REPS)
-    print("static band %4d int%d: %d windows, resident %d, kernel %.2f ms, cells %.3e" % (band, score, n, b.resident_windows, ms, b.last_cells()))
+    print("%s %s %4d int%d: %d windows, resident %d, kernel %.2f ms, cells %.3e" % (kernel, mode, band, score, n, b.resident_windows, ms, b.last_cells()))
     b.close()
 
 
 if __name__ == "__main__":
     p = torch.cuda.get_device_properties(0)
     print("device:", p.name, p.multi_processor_count, "SMs")
-    c3()
+    if "--no-c3" not in sys.argv:
+        c3()
     if "--no-static" not in sys.argv:
         for band in (512, 1024, 1536):
             for score in (16, 32):
                 static_band(band, score)
+    for score in (16, 32):
+        static_band(2048, score, kernel="v1")
+        for band in (256, 1536):
+            static_band(band, score, "static_band_traceback", "tb")
     torch.cuda.empty_cache()
