@@ -15,7 +15,8 @@
 //       int16 scores, backtrace preference insertion, deletion, diagonal; query / target swapped when the query is longer),
 //       aligner_global_ukkonen.cpp:30-81.
 // Pinned against: the CIGAR tables of Test_AlignerGlobal.cpp:78-147 and test_cudaaligner_bindings.py (tests/test_oracle_global.py)
-// and, on the GPU box, the unmodified reference classes through oracle/_ref (tests/test_gpu_global_aligners.py).
+// and, on the GPU box, the unmodified reference classes through oracle/_ref (tests/test_gpu_global_aligners.py,
+// tests/test_gpu_global_kernel_paths.py: skewed shapes, small max_query_length, long queries, wide Ukkonen bands).
 #include <algorithm>
 #include <climits>
 #include <cstdint>
@@ -114,10 +115,25 @@ struct Range
     int32_t qb, qe, tb, te;
 };
 
+// What one Hirschberg alignment ran (oracle_global_stats): DP cells counted the way the kernel counts them, and the decisions
+// that depend on max_query_length or on the midpoint rule
+struct HirschbergStats
+{
+    int64_t cells            = 0; // leaf: ql x tl; split: ql x tl (both half passes); empty and single-character slices: 0
+    int64_t leaves           = 0;
+    int64_t splits           = 0;
+    int64_t short_splits     = 0; // splits of a slice with ql < full_myers_threshold whose matrix did not fit
+    int64_t single_char_long = 0; // single-character slices with tl > 32 (more than one lane's worth of target)
+    int64_t tied_splits      = 0; // the minimum score sum is attained at two or more target positions
+    int64_t lane_rule_splits = 0; // the stride-32 lane rule picks another position than the smallest minimising one
+};
+
 // hirschberg_myers (hirschberg_myers_gpu.cu:575-644). Returns false when the 64-entry stack overflows.
 bool hirschberg(const char* query, int32_t query_length, const char* target, int32_t target_length, int32_t full_myers_threshold,
-                int64_t max_elements_per_matrix, int32_t stack_capacity, std::vector<int8_t>& path)
+                int64_t max_elements_per_matrix, int32_t stack_capacity, std::vector<int8_t>& path, HirschbergStats* stats = nullptr)
 {
+    HirschbergStats ignored;
+    HirschbergStats& st = stats ? *stats : ignored;
     std::vector<Range> stack;
     stack.push_back({0, query_length, 0, target_length});
     std::vector<int32_t> fwd, rev;
@@ -137,6 +153,8 @@ bool hirschberg(const char* query, int32_t query_length, const char* target, int
         else if (ql == 1)
         {
             // hirschberg_myers_single_char_warp (:483-519)
+            if (tl > 32)
+                st.single_char_long++;
             const char qc = query[e.qb];
             int32_t t     = e.te - 1;
             bool matched  = false;
@@ -168,9 +186,14 @@ bool hirschberg(const char* query, int32_t query_length, const char* target, int
                 if (static_cast<int64_t>(tl + 1) * n_words <= max_elements_per_matrix)
                 {
                     full_matrix_path(query + e.qb, ql, target + e.tb, tl, path);
+                    st.cells += static_cast<int64_t>(ql) * tl;
+                    st.leaves++;
                     continue;
                 }
+                st.short_splits++;
             }
+            st.cells += static_cast<int64_t>(ql) * tl;
+            st.splits++;
             const int32_t qm = e.qb + ql / 2;
             // hirschberg_myers_compute_target_mid_warp (:412-481)
             last_row_scores(query + e.qb, qm - e.qb, target + e.tb, tl, false, fwd);
@@ -208,6 +231,25 @@ bool hirschberg(const char* query, int32_t query_length, const char* target, int
                     }
                 }
             }
+            int32_t best = INT_MAX, first = 0, n_best = 0;
+            for (int32_t t = 0; t <= tl; t++)
+            {
+                const int32_t sum = fwd[t] + rev[tl - t];
+                if (sum < best)
+                {
+                    best   = sum;
+                    first  = t;
+                    n_best = 1;
+                }
+                else if (sum == best)
+                {
+                    n_best++;
+                }
+            }
+            if (n_best > 1)
+                st.tied_splits++;
+            if (mid[0] != first)
+                st.lane_rule_splits++;
             const int32_t tm = e.tb + mid[0];
             if (static_cast<int32_t>(stack.size()) >= stack_capacity)
                 return false;
@@ -366,6 +408,37 @@ int32_t oracle_ukkonen_align(const char* query, int32_t query_length, const char
     std::reverse(path.begin(), path.end());
     std::memcpy(actions, path.data(), path.size());
     return static_cast<int32_t>(path.size());
+}
+
+// What one alignment of `algorithm` (0 Hirschberg-Myers at max_query_length, 1 unbanded Myers, 2 Ukkonen with p = 100) runs.
+// out[7]: DP cells as the kernels count them, then for Hirschberg-Myers leaves, splits, short splits (query slice below the
+// full-matrix threshold whose matrix did not fit), single-character slices over more than 32 target bases, splits whose minimum
+// score sum is tied, splits where the lane rule picks another target position than the smallest minimising one. Returns 1 when
+// the Hirschberg stack overflowed, else 0.
+int32_t oracle_global_stats(int32_t algorithm, const char* query, int32_t query_length, const char* target, int32_t target_length,
+                            int32_t max_query_length, int64_t* out)
+{
+    HirschbergStats st;
+    int32_t failed = 0;
+    if (algorithm == 0)
+    {
+        std::vector<int8_t> path;
+        const int64_t max_el = static_cast<int64_t>((max_query_length + 31) / 32) * 64;
+        failed               = hirschberg(query, query_length, target, target_length, 63, max_el, 64, path, &st) ? 0 : 1;
+    }
+    else if (algorithm == 1)
+    {
+        st.cells = static_cast<int64_t>(query_length) * target_length;
+    }
+    else
+    {
+        // bw x (n + m) slots after the swap (m <= n), as ukkonen() lays them out
+        const int32_t m = std::min(query_length, target_length) + 1, n = std::max(query_length, target_length) + 1;
+        st.cells        = static_cast<int64_t>((1 + n - m + 2 * 100 + 1) / 2) * (n + m);
+    }
+    const int64_t v[7] = {st.cells, st.leaves, st.splits, st.short_splits, st.single_char_long, st.tied_splits, st.lane_rule_splits};
+    std::memcpy(out, v, sizeof(v));
+    return failed;
 }
 
 } // extern "C"

@@ -265,6 +265,25 @@ def myers_full_align(query, target):
     return out[:n].copy()
 
 
+GLOBAL_STATS = ("cells", "leaves", "splits", "short_splits", "single_char_long", "tied_splits", "lane_rule_splits")
+
+
+def global_stats(algorithm, query, target, max_query_length=None):
+    """What one alignment of a fixed-size global aligner ("hirschberg_myers" at max_query_length, "myers", "ukkonen") runs: the DP
+    cells as the kernels count them (GlobalAligner.last_cells sums them over a batch) and, for Hirschberg-Myers, its leaf / split
+    decisions and midpoint ties -> dict over GLOBAL_STATS plus "failed"."""
+    q = query.encode() if isinstance(query, str) else bytes(query)
+    t = target.encode() if isinstance(target, str) else bytes(target)
+    mq = len(q) if max_query_length is None else max_query_length
+    alg = {"hirschberg_myers": 0, "myers": 1, "ukkonen": 2}[algorithm]
+    out = np.zeros(len(GLOBAL_STATS), dtype=np.int64)
+    lib().oracle_global_stats.restype = C.c_int32
+    failed = lib().oracle_global_stats(C.c_int32(alg), q, C.c_int32(len(q)), t, C.c_int32(len(t)), C.c_int32(mq), _p(out, C.c_int64))
+    res = {k: int(v) for k, v in zip(GLOBAL_STATS, out)}
+    res["failed"] = bool(failed)
+    return res
+
+
 def ukkonen_align(query, target, p=100):
     """AlignerGlobalUkkonen (fixed p = 100) -> states ndarray."""
     q = query.encode() if isinstance(query, str) else bytes(query)
