@@ -13,6 +13,7 @@
 
 #include <algorithm>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <thread>
 #include <vector>
@@ -47,103 +48,6 @@ enum class PoaKernel
     v1, // poa_window_kernel: wider bands and reads of 64 k bases and more
 };
 
-// The v3 kernel packs band starts in 16 bits; only the traceback kernel hosts the traceback-matrix alignment.
-PoaKernel select_kernel(const gwb200_poa_config& c)
-{
-    if (c.band_mode == GWB200_POA_STATIC_BAND_TRACEBACK || c.band_mode == GWB200_POA_ADAPTIVE_BAND_TRACEBACK)
-        return PoaKernel::tb;
-    if (c.alignment_band_width <= kMaxAdaptiveBW && c.max_sequence_size < 65536)
-        return PoaKernel::v3;
-    return PoaKernel::v1;
-}
-
-struct Carver
-{
-    uint8_t* base;
-    int64_t off = 0;
-    template <typename T>
-    T* take(int64_t count)
-    {
-        off      = align_up64(off, 256);
-        T* p     = reinterpret_cast<T*>(base + off);
-        off += count * static_cast<int64_t>(sizeof(T));
-        return p;
-    }
-};
-
-} // namespace
-
-struct gwb200_poa_batch
-{
-    int32_t device_id = 0;
-    cudaStream_t stream = nullptr;
-    int8_t output_mask  = 0;
-    gwb200_poa_config cfg{};
-    int32_t gap = -8, mismatch = -6, match = 8;
-    bool score32 = false, size32 = false, msa = false;
-    bool accurate = false; // SPOA_ACCURATE semantics (racon sort after every read)
-    int32_t score_bytes = 2, size_bytes = 2;
-    int32_t bid = 0;
-
-    int32_t max_poas = 0;
-    int32_t poa_count = 0;
-    int32_t num_nucleotides_copied = 0;
-    int32_t global_sequence_idx = 0;
-    int64_t avail_buf_mem = 0, scorebuf_alloc_size = 0;
-    int64_t next_scores_offset = 0;
-    int64_t seq_capacity = 0; // bytes in the sequences / weights buffers (without slack)
-
-    // pinned host
-    PinnedBuf<uint8_t> h_block;
-    uint8_t* h_sequences = nullptr;
-    int8_t* h_weights = nullptr;
-    bool weights_present = false; // false: every read so far had unit base weights (h_weights is not filled, the device array is memset)
-    struct CopyJob
-    {
-        uint8_t* dst;
-        const char* src;
-        int32_t len;
-    };
-    std::vector<CopyJob>* deferred = nullptr; // set by add_groups_flat: sequence copies are collected and run on several threads
-    int32_t* h_seq_lengths = nullptr;
-    WindowInfo* h_windows = nullptr;
-    uint8_t* h_consensus = nullptr;
-    uint16_t* h_coverage = nullptr;
-    int32_t* h_cons_len = nullptr;
-    int32_t* h_status = nullptr;
-    int32_t* h_node_count = nullptr;
-    unsigned long long* h_cells = nullptr;
-    uint8_t* h_msa = nullptr;
-
-    // device
-    uint8_t* d_block = nullptr;
-    bool owns_dblock = true; // false: the block belongs to the caller's allocator (create_batch overload with an allocator)
-    DeviceParams P{};
-    V2Extra X{};
-    PoaKernel kernel = PoaKernel::v3;
-    bool tb_mode = false;    // static_band_traceback / adaptive_band_traceback
-    int32_t trace_bytes = 2; // sizeof(TraceT): 1 unless max_banded_pred_distance > 127 (cudapoa_limits.hpp:56-60)
-    bool timers_on = false;
-    unsigned long long* d_timers = nullptr;
-
-    EventTimer timer;
-    bool launched = false;
-    bool results_on_host = false;
-
-    static int32_t batches;
-};
-int32_t gwb200_poa_batch::batches = 0;
-
-namespace
-{
-
-struct Sizes
-{
-    int64_t dev_per_poa = 0, dev_per_matrix = 0, host_per_poa = 0;
-    int64_t seq_bytes_per_poa = 0;
-    int32_t aln_capacity = 0, stack_capacity = 0;
-};
-
 // SPOA_ACCURATE as a library-wide switch (the reference makes it a build flag, cudapoa_kernels.cuh:508-520): batches created while
 // it is on re-sort their graphs with racon's topological sort after every read
 std::atomic<int> g_spoa_accurate{-1};
@@ -158,55 +62,227 @@ bool spoa_accurate()
     return v != 0;
 }
 
-Sizes compute_sizes(const gwb200_poa_config& c, int32_t score_bytes, int32_t sz, bool msa, bool tb = false, int32_t trace_bytes = 2)
+// What the config, the scores and the output type decide about a batch
+struct BatchShape
 {
-    Sizes s;
-    const int64_t mn = c.max_nodes_per_graph;
-    const int64_t E  = kMaxEdges;
-    s.aln_capacity   = c.max_nodes_per_graph + c.max_sequence_size + 16;
-    const bool accurate = spoa_accurate();
-    s.stack_capacity = (msa || accurate) ? 4 * c.max_nodes_per_graph + 16 : 0;
-    s.seq_bytes_per_poa = static_cast<int64_t>(c.max_sequences_per_poa) * align_up(std::max(c.max_sequence_size, 1), 4);
-    int64_t d = 0;
-    d += mn * 1;                 // nodes
-    d += mn * 2 * 5;             // in_cnt out_cnt aln_cnt cov local_cnt
-    d += mn * E * sz * 2;        // in_edges, out_edges
-    d += mn * kMaxAligned * sz;  // aligned
-    d += mn * E * 2;             // in_w
-    d += mn * sz * 2;            // sorted, pos
-    d += 2ll * s.aln_capacity * sz;
-    d += mn * 4 + mn * sz;       // consensus scratch
-    d += s.seq_bytes_per_poa * 2;              // sequences + weights
-    d += 4ll * c.max_sequences_per_poa;        // seq lengths
-    d += sizeof(WindowInfo);
-    d += c.max_consensus_size * 3ll;           // consensus + coverage
-    d += 4 * 3 + 8;                            // len, status, node_count, cells
-    if (msa)
-    {
-        d += s.seq_bytes_per_poa * sz; // path
-        d += mn * sz + mn * 2;         // msa_col, marks, check
-        d += static_cast<int64_t>(s.stack_capacity) * sz;
-        d += static_cast<int64_t>(c.max_sequences_per_poa) * c.max_consensus_size;
-    }
-    else if (accurate)
-    {
-        d += mn * 2 + static_cast<int64_t>(s.stack_capacity) * sz; // marks, check, stack of the racon sort
-    }
-    d += (mn + 1) * 16;                                   // v2 row metadata
-    d += (align_up(std::max(c.max_sequence_size, 1), 4) + 8ll) * sz; // v2 read -> node map
-    d += 64;                                             // phase timers
-    d += 256 * 36; // carving alignment slack
-    if (tb)
-        d += static_cast<int64_t>(c.matrix_sequence_dimension) * c.max_banded_pred_distance * score_bytes + 256; // score ring (allocate_block.hpp:333-334,374)
-    s.dev_per_poa    = d;
-    // the pooled matrix: scores, or the trace matrix in the traceback modes (allocate_block.hpp:76-84)
-    s.dev_per_matrix = static_cast<int64_t>(c.matrix_sequence_dimension) * mn * (tb ? trace_bytes : score_bytes);
-    int64_t h        = s.seq_bytes_per_poa * 2 + 4ll * c.max_sequences_per_poa + sizeof(WindowInfo) + c.max_consensus_size * 3ll + 4 * 3 + 8;
-    if (msa)
-        h += static_cast<int64_t>(c.max_sequences_per_poa) * c.max_consensus_size;
-    s.host_per_poa = h + 64;
+    int32_t score_bytes; // sizeof(ScoreT)
+    int32_t size_bytes;  // sizeof(SizeT): node and read indices
+    bool tb;             // static_band_traceback / adaptive_band_traceback
+    int32_t trace_bytes; // sizeof(TraceT): 1 unless max_banded_pred_distance > 127 (cudapoa_limits.hpp:56-60)
+    bool msa;
+    bool accurate; // SPOA_ACCURATE semantics (racon sort after every read)
+    PoaKernel kernel;
+};
+
+BatchShape batch_shape(const gwb200_poa_config& c, int32_t gap, int32_t mismatch, int32_t match, int8_t output_mask)
+{
+    BatchShape s;
+    s.score_bytes = use32bit_score(c, gap, mismatch, match) ? 4 : 2;
+    s.size_bytes  = use32bit_size(c) ? 4 : 2;
+    s.tb          = c.band_mode == GWB200_POA_STATIC_BAND_TRACEBACK || c.band_mode == GWB200_POA_ADAPTIVE_BAND_TRACEBACK;
+    s.trace_bytes = c.max_banded_pred_distance > INT8_MAX ? 2 : 1;
+    s.msa         = (output_mask & GWB200_POA_OUTPUT_MSA) != 0;
+    s.accurate    = spoa_accurate();
+    // the v3 kernel packs band starts in 16 bits; only the traceback kernel hosts the traceback-matrix alignment
+    if (s.tb)
+        s.kernel = PoaKernel::tb;
+    else if (c.alignment_band_width <= kMaxAdaptiveBW && c.max_sequence_size < 65536)
+        s.kernel = PoaKernel::v3;
+    else
+        s.kernel = PoaKernel::v1;
     return s;
 }
+
+// Slack of the arena layout. Every batch's max_poas and score pool depend on these numbers.
+constexpr int64_t kSeqTail           = 4096;                    // past the last read of the sequences / weights arrays
+constexpr int64_t kDeviceWindowSlack = 256 * 36;                // per window: the 256-byte alignment of the device arrays
+constexpr int64_t kDeviceReserve     = kSeqTail * 2 + 256 * 64; // per batch: the sequence tails and the rest of the alignment
+constexpr int64_t kHostWindowSlack   = 64;                      // per window: the alignment of the host arrays
+constexpr int64_t kHostReserve       = kSeqTail * 2 + 4096;     // per batch: the sequence tails and the rest of the alignment
+
+// One pass over the arrays of a block in carve order: each starts 256-byte aligned and holds `per_window` elements per window
+// plus `fixed`. `window` sums the bytes one window adds. Without a base the pass only measures.
+struct Arena
+{
+    uint8_t* base  = nullptr;
+    int64_t n      = 0; // windows
+    int64_t off    = 0; // end of the carve
+    int64_t window = 0;
+
+    template <typename T>
+    T* take(int64_t per_window, int64_t fixed = 0)
+    {
+        const int64_t bytes = sizeof(T);
+        window += per_window * bytes;
+        off  = align_up64(off, 256);
+        T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+        off += (n * per_window + fixed) * bytes;
+        return p;
+    }
+};
+
+// Every array of a batch: the pinned host mirrors and the arrays of the device block
+struct PoaArrays
+{
+    uint8_t* h_sequences = nullptr;
+    int8_t* h_weights    = nullptr;
+    int32_t* h_seq_lengths = nullptr;
+    WindowInfo* h_windows  = nullptr;
+    uint8_t* h_consensus   = nullptr;
+    uint16_t* h_coverage   = nullptr;
+    int32_t* h_cons_len    = nullptr;
+    int32_t* h_status      = nullptr;
+    int32_t* h_node_count  = nullptr;
+    unsigned long long* h_cells = nullptr;
+    uint8_t* h_msa              = nullptr;
+
+    DeviceParams P{};
+    V2Extra X{};
+    unsigned long long* d_timers = nullptr;
+};
+
+// Bases of one window's reads in the sequences array, each read padded to 4
+int64_t window_bases(const gwb200_poa_config& c)
+{
+    return static_cast<int64_t>(c.max_sequences_per_poa) * align_up(std::max(c.max_sequence_size, 1), 4);
+}
+
+// The one list of a batch's arrays, in carve order: the pinned host block `h`, then the device block `d`. What the device list
+// leaves of its block is the score pool.
+void lay_out(Arena& h, Arena& d, const BatchShape& s, const gwb200_poa_config& c, PoaArrays& a)
+{
+    const int64_t mn = c.max_nodes_per_graph, mc = c.max_consensus_size, ms = c.max_sequences_per_poa, S = s.size_bytes;
+    const int64_t bases = window_bases(c);
+    DeviceParams& P     = a.P;
+    V2Extra& X          = a.X;
+    P.aln_capacity      = c.max_nodes_per_graph + c.max_sequence_size + 16;
+    P.stack_capacity    = (s.msa || s.accurate) ? 4 * c.max_nodes_per_graph + 16 : 0;
+    X.rd_capacity       = align_up(std::max(c.max_sequence_size, 1), 4) + 8;
+
+    a.h_sequences   = h.take<uint8_t>(bases, kSeqTail);
+    a.h_weights     = h.take<int8_t>(bases, kSeqTail);
+    a.h_seq_lengths = h.take<int32_t>(ms);
+    a.h_windows     = h.take<WindowInfo>(1);
+    a.h_consensus   = h.take<uint8_t>(mc);
+    a.h_coverage    = h.take<uint16_t>(mc);
+    a.h_cons_len    = h.take<int32_t>(1);
+    a.h_status      = h.take<int32_t>(1);
+    a.h_node_count  = h.take<int32_t>(1);
+    a.h_cells       = h.take<unsigned long long>(1);
+    if (s.msa)
+        a.h_msa = h.take<uint8_t>(ms * mc);
+
+    P.sequences     = d.take<uint8_t>(bases, kSeqTail);
+    P.weights       = d.take<int8_t>(bases, kSeqTail);
+    P.seq_lengths   = d.take<int32_t>(ms);
+    P.windows       = d.take<WindowInfo>(1);
+    P.nodes         = d.take<uint8_t>(mn);
+    P.in_cnt        = d.take<uint16_t>(mn);
+    P.out_cnt       = d.take<uint16_t>(mn);
+    P.aln_cnt       = d.take<uint16_t>(mn);
+    P.node_cov      = d.take<uint16_t>(mn);
+    P.local_cnt     = d.take<uint16_t>(mn);
+    P.in_edges      = d.take<uint8_t>(mn * kMaxEdges * S);
+    P.out_edges     = d.take<uint8_t>(mn * kMaxEdges * S);
+    P.aligned       = d.take<uint8_t>(mn * kMaxAligned * S);
+    P.in_w          = d.take<uint16_t>(mn * kMaxEdges);
+    P.sorted        = d.take<uint8_t>(mn * S);
+    P.pos           = d.take<uint8_t>(mn * S);
+    P.aln_graph     = d.take<uint8_t>(P.aln_capacity * S);
+    P.aln_read      = d.take<uint8_t>(P.aln_capacity * S);
+    P.cons_scores   = d.take<int32_t>(mn);
+    P.cons_preds    = d.take<uint8_t>(mn * S);
+    P.consensus     = d.take<uint8_t>(mc);
+    P.coverage      = d.take<uint16_t>(mc);
+    P.consensus_len = d.take<int32_t>(1);
+    P.status        = d.take<int32_t>(1);
+    P.node_count    = d.take<int32_t>(1);
+    P.cells         = d.take<unsigned long long>(1);
+    if (s.msa)
+    {
+        P.seq_path = d.take<uint8_t>(bases * S, kSeqTail * S);
+        P.msa_col  = d.take<uint8_t>(mn * S);
+    }
+    if (s.msa || s.accurate) // the MSA and the racon sort
+    {
+        P.marks = d.take<uint8_t>(mn);
+        P.check = d.take<uint8_t>(mn);
+        P.stack = d.take<uint8_t>(P.stack_capacity * S);
+    }
+    if (s.msa)
+        P.msa_out = d.take<uint8_t>(ms * mc);
+    X.row_meta     = d.take<int4>(mn + 1);
+    X.rd_node      = d.take<uint8_t>(X.rd_capacity * S);
+    a.d_timers     = d.take<unsigned long long>(8);
+    X.work_counter = d.take<int32_t>(0, 64);
+    if (s.tb) // score ring (allocate_block.hpp:333-334,374)
+        X.tb_scores = d.take<uint8_t>(static_cast<int64_t>(c.matrix_sequence_dimension) * c.max_banded_pred_distance * s.score_bytes + 256);
+}
+
+// Bytes one window needs: on the host, on the device besides its matrix, and its matrix in the score pool (scores, or the trace
+// matrix in the traceback modes, allocate_block.hpp:76-84)
+struct WindowBytes
+{
+    int64_t host, device, matrix;
+};
+
+WindowBytes window_bytes(const BatchShape& s, const gwb200_poa_config& c)
+{
+    Arena h, d;
+    PoaArrays unused;
+    lay_out(h, d, s, c, unused);
+    return {h.window + kHostWindowSlack, d.window + kDeviceWindowSlack,
+            static_cast<int64_t>(c.matrix_sequence_dimension) * c.max_nodes_per_graph * (s.tb ? s.trace_bytes : s.score_bytes)};
+}
+
+struct CudaFree
+{
+    void operator()(void* p) const { cudaFree(p); }
+};
+
+} // namespace
+
+struct gwb200_poa_batch : PoaArrays
+{
+    int32_t device_id = 0;
+    cudaStream_t stream = nullptr;
+    int8_t output_mask  = 0;
+    gwb200_poa_config cfg{};
+    int32_t gap = -8, mismatch = -6, match = 8;
+    BatchShape shape{};
+    int32_t bid = 0;
+
+    int32_t max_poas = 0;
+    int32_t poa_count = 0;
+    int32_t num_nucleotides_copied = 0;
+    int32_t global_sequence_idx = 0;
+    int64_t avail_buf_mem = 0, scorebuf_alloc_size = 0;
+    int64_t next_scores_offset = 0;
+
+    PinnedBuf<uint8_t> h_block;
+    bool weights_present = false; // false: every read so far had unit base weights (h_weights is not filled, the device array is memset)
+    struct CopyJob
+    {
+        uint8_t* dst;
+        const char* src;
+        int32_t len;
+    };
+    std::vector<CopyJob>* deferred = nullptr; // set by add_groups_flat: sequence copies are collected and run on several threads
+
+    // the device block when the batch allocated it; a caller's block (gwb200_poa_batch_create_in_block) is not the batch's to free
+    std::unique_ptr<uint8_t, CudaFree> d_block;
+    bool timers_on = false;
+
+    EventTimer timer;
+    bool launched = false;
+    bool results_on_host = false;
+
+    static int32_t batches;
+};
+int32_t gwb200_poa_batch::batches = 0;
+
+namespace
+{
 
 // Dynamic shared memory per CTA of the v3 kernel. The resident windows of one SM share its 227 KB: the pool is what one CTA gets
 // when the batch's capacity (HBM) is spread over the SMs, at most 16 CTAs per SM (registers) -- a batch that HBM limits to a
@@ -218,9 +294,10 @@ int32_t v3_pool_bytes(const gwb200_poa_batch* b)
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, b->device_id);
     int smem_sm = 233472;
     cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, b->device_id);
+    const bool score32    = b->shape.score_bytes == 4;
     const int32_t ctas    = static_cast<int32_t>(std::min<int64_t>(16, std::max<int64_t>(1, (static_cast<int64_t>(b->max_poas) + sms - 1) / sms)));
     const int64_t max_bw  = (b->cfg.band_mode == GWB200_POA_ADAPTIVE_BAND) ? kMaxAdaptiveBW : b->cfg.alignment_band_width;
-    const int64_t need    = std::max<int64_t>(2 * (max_bw + 8) * b->score_bytes, 2 * (b->score32 ? TileBuf<int32_t>::kBytes : TileBuf<int16_t>::kBytes));
+    const int64_t need    = std::max<int64_t>(2 * (max_bw + 8) * b->shape.score_bytes, 2 * (score32 ? TileBuf<int32_t>::kBytes : TileBuf<int16_t>::kBytes));
     const int64_t statics = sizeof(V3Shared) + 64;
     int64_t pool          = smem_sm / ctas - 1024 - statics;
     pool                  = std::min<int64_t>(pool, 96 * 1024) / 256 * 256;
@@ -235,8 +312,8 @@ int32_t v3_pool_bytes(const gwb200_poa_batch* b)
 int32_t tb_pool_bytes(const gwb200_poa_batch* b)
 {
     const int64_t bw   = b->cfg.alignment_band_width;
-    const int64_t dflt = b->score32 ? 24 * 1024 : 12 * 1024;
-    const int64_t need = (b->cfg.max_sequence_size + bw + 24) + 2 * (bw + 8) * b->score_bytes;
+    const int64_t dflt = b->shape.score_bytes == 4 ? 24 * 1024 : 12 * 1024;
+    const int64_t need = (b->cfg.max_sequence_size + bw + 24) + 2 * (bw + 8) * b->shape.score_bytes;
     return static_cast<int32_t>(std::max<int64_t>(dflt, align_up64(need, 1024)));
 }
 
@@ -246,15 +323,51 @@ int32_t tb_pool_bytes(const gwb200_poa_batch* b)
 // the largest carve-out (28 KB of L1 left) it ran 10-15 % slower at static band 2048 on an H100.
 constexpr int32_t kV1PoolBytes = 1024;
 
-// Resident CTAs per SM of a one-warp kernel with `smem` bytes of dynamic shared memory, after making that pool size launchable.
-// The kernel's residency is sized against the carve-out asked for here (the full one unless the caller needs less shared memory);
-// do not inherit a device-wide cache preference another library set in this process (the reference does cudaDeviceSetCacheConfig(PreferL1), cudapoa_kernels.cuh:605).
-template <typename Kernel>
-int32_t pooled_occupancy(Kernel kfn, int32_t smem, int32_t carveout = cudaSharedmemCarveoutMaxShared)
+int32_t pool_bytes(const gwb200_poa_batch* b)
 {
+    switch (b->shape.kernel)
+    {
+    case PoaKernel::v3: return v3_pool_bytes(b);
+    case PoaKernel::tb: return tb_pool_bytes(b);
+    default: return kV1PoolBytes;
+    }
+}
+
+using WindowKernel = void (*)(const DeviceParams, const V2Extra);
+
+template <typename ScoreT, typename SizeT>
+WindowKernel typed_kernel(PoaKernel k)
+{
+    WindowKernel kfn = poa_window_kernel<ScoreT, SizeT>;
+    if (k == PoaKernel::v3)
+        kfn = poa_window_kernel_v3<ScoreT, SizeT>;
+    else if (k == PoaKernel::tb)
+        kfn = poa_window_kernel_tb<ScoreT, SizeT>;
+    return kfn;
+}
+
+// The batch's kernel, instantiated for its score and index widths
+WindowKernel window_kernel(const gwb200_poa_batch* b)
+{
+    const bool score32 = b->shape.score_bytes == 4, size32 = b->shape.size_bytes == 4;
+    if (!score32 && !size32)
+        return typed_kernel<int16_t, int16_t>(b->shape.kernel);
+    if (score32 && !size32)
+        return typed_kernel<int32_t, int16_t>(b->shape.kernel);
+    return typed_kernel<int32_t, int32_t>(b->shape.kernel);
+}
+
+// Resident CTAs per SM of the batch's kernel with its pool of dynamic shared memory, after making that pool launchable. The
+// kernel's residency is sized against the carve-out asked for here (the full one; the first-generation kernel leaves it to the
+// driver): do not inherit a device-wide cache preference another library set in this process (the reference does
+// cudaDeviceSetCacheConfig(PreferL1), cudapoa_kernels.cuh:605).
+int32_t resident_ctas(const gwb200_poa_batch* b, WindowKernel kfn)
+{
+    const int32_t smem = b->X.pool_bytes;
     if (smem > 48 * 1024)
         cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    cudaFuncSetAttribute(kfn, cudaFuncAttributePreferredSharedMemoryCarveout, carveout);
+    cudaFuncSetAttribute(kfn, cudaFuncAttributePreferredSharedMemoryCarveout,
+                         b->shape.kernel == PoaKernel::v1 ? cudaSharedmemCarveoutDefault : cudaSharedmemCarveoutMaxShared);
     int nb = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kfn, 32, smem) != cudaSuccess)
     {
@@ -262,44 +375,6 @@ int32_t pooled_occupancy(Kernel kfn, int32_t smem, int32_t carveout = cudaShared
         nb = 0;
     }
     return nb;
-}
-
-// action 0: launch; action 1: return resident CTAs per SM (occupancy) of the batch's kernel
-template <typename ScoreT, typename SizeT>
-int32_t typed_action(gwb200_poa_batch* b, int action)
-{
-    void (*kfn)(const DeviceParams, const V2Extra) = poa_window_kernel<ScoreT, SizeT>;
-    if (b->kernel == PoaKernel::v3)
-        kfn = poa_window_kernel_v3<ScoreT, SizeT>;
-    else if (b->kernel == PoaKernel::tb)
-        kfn = poa_window_kernel_tb<ScoreT, SizeT>;
-    const int32_t smem = b->X.pool_bytes;
-    const int32_t nb   = b->kernel == PoaKernel::v1 ? pooled_occupancy(kfn, smem, cudaSharedmemCarveoutDefault) : pooled_occupancy(kfn, smem);
-    if (action == 1)
-        return nb;
-    b->X.timers = b->timers_on ? b->d_timers : nullptr;
-    if (b->timers_on)
-        cudaMemsetAsync(b->d_timers, 0, sizeof(unsigned long long) * 8 * b->poa_count, b->stream);
-    int32_t grid = b->poa_count;
-    if (b->kernel == PoaKernel::v3)
-    {
-        int sms = 132;
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, b->device_id);
-        grid = std::max(1, std::min(b->poa_count, std::max(1, nb) * sms));
-        cudaMemsetAsync(b->X.work_counter, 0, sizeof(int32_t), b->stream);
-    }
-    kfn<<<grid, 32, smem, b->stream>>>(b->P, b->X);
-    count_launch();
-    return 0;
-}
-
-int32_t batch_action(gwb200_poa_batch* b, int action)
-{
-    if (!b->score32 && !b->size32)
-        return typed_action<int16_t, int16_t>(b, action);
-    if (b->score32 && !b->size32)
-        return typed_action<int32_t, int16_t>(b, action);
-    return typed_action<int32_t, int32_t>(b, action);
 }
 
 int validate_config(const gwb200_poa_config& c)
@@ -476,11 +551,9 @@ int64_t gwb200_poa_estimate_max_poas(const gwb200_poa_config* cfg, int32_t msa_f
         cudaGetLastError();
         return set_error(GWB200_E_CUDA, "no usable CUDA device: this engine has no CPU fallback");
     }
-    const int32_t score_bytes = use32bit_score(*cfg, gap_score, mismatch_score, match_score) ? 4 : 2;
-    const int32_t size_bytes  = use32bit_size(*cfg) ? 4 : 2;
-    const bool tb             = cfg->band_mode == GWB200_POA_STATIC_BAND_TRACEBACK || cfg->band_mode == GWB200_POA_ADAPTIVE_BAND_TRACEBACK;
-    const Sizes sz            = compute_sizes(*cfg, score_bytes, size_bytes, msa_flag != 0, tb, cfg->max_banded_pred_distance > INT8_MAX ? 2 : 1);
-    const int64_t per         = sz.dev_per_poa + sz.dev_per_matrix;
+    const BatchShape s  = batch_shape(*cfg, gap_score, mismatch_score, match_score, msa_flag ? GWB200_POA_OUTPUT_MSA : GWB200_POA_OUTPUT_CONSENSUS);
+    const WindowBytes w = window_bytes(s, *cfg);
+    const int64_t per   = w.device + w.matrix;
     if (per <= 0)
         return 0;
     return static_cast<int64_t>(static_cast<double>(gpu_memory_usage_quota) * static_cast<double>(free_b)) / per;
@@ -523,196 +596,93 @@ static int poa_batch_create_impl(gwb200_poa_batch** out, int32_t device_id, void
         return rc;
     DeviceGuard guard(device_id);
 
-    gwb200_poa_batch* b = new gwb200_poa_batch;
-    b->device_id        = device_id;
-    b->stream           = static_cast<cudaStream_t>(stream);
-    b->output_mask      = output_mask;
-    b->cfg              = *cfg;
-    b->gap              = gap_score;
-    b->mismatch         = mismatch_score;
-    b->match            = match_score;
-    b->score32          = use32bit_score(*cfg, gap_score, mismatch_score, match_score);
-    b->size32           = use32bit_size(*cfg);
-    b->score_bytes      = b->score32 ? 4 : 2;
-    b->size_bytes       = b->size32 ? 4 : 2;
-    b->msa              = (output_mask & GWB200_POA_OUTPUT_MSA) != 0;
-    b->accurate         = spoa_accurate();
-    b->tb_mode          = cfg->band_mode == GWB200_POA_STATIC_BAND_TRACEBACK || cfg->band_mode == GWB200_POA_ADAPTIVE_BAND_TRACEBACK;
-    b->trace_bytes      = cfg->max_banded_pred_distance > INT8_MAX ? 2 : 1;
-    if (b->tb_mode && cfg->max_banded_pred_distance < 1)
-    {
-        delete b;
+    std::unique_ptr<gwb200_poa_batch> b(new gwb200_poa_batch);
+    b->device_id   = device_id;
+    b->stream      = static_cast<cudaStream_t>(stream);
+    b->output_mask = output_mask;
+    b->cfg         = *cfg;
+    b->gap         = gap_score;
+    b->mismatch    = mismatch_score;
+    b->match       = match_score;
+    b->shape       = batch_shape(*cfg, gap_score, mismatch_score, match_score, output_mask);
+    if (b->shape.tb && cfg->max_banded_pred_distance < 1)
         return set_error(GWB200_E_INVALID_ARGUMENT, "max_banded_pred_distance has to be positive in the traceback band modes");
-    }
-    b->bid              = gwb200_poa_batch::batches++;
-    b->kernel           = select_kernel(*cfg);
+    b->bid = gwb200_poa_batch::batches++;
 
     size_t free_b = 0, total_b = 0;
     if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess)
-    {
-        delete b;
         return set_error(GWB200_E_CUDA, "cudaMemGetInfo failed");
-    }
     int64_t avail = static_cast<int64_t>(static_cast<double>(free_b) * 0.95);
     if (max_gpu_mem >= 0)
         avail = std::min(avail, max_gpu_mem);
-    const int64_t fixed_dev = 4096 * 2 + 256 * 64; // per-batch constant part of the device block
     if (ext_block)
-        avail = ext_bytes - fixed_dev; // the caller's block is the budget: everything has to fit inside it
-    const Sizes sz = compute_sizes(*cfg, b->score_bytes, b->size_bytes, b->msa, b->tb_mode, b->trace_bytes);
-    if (avail < sz.dev_per_poa + (cfg->band_mode == GWB200_POA_FULL_BAND ? 0 : sz.dev_per_matrix) || sz.dev_per_poa + sz.dev_per_matrix <= 0)
+        avail = ext_bytes - kDeviceReserve; // the caller's block is the budget: everything has to fit inside it
+    const WindowBytes w = window_bytes(b->shape, *cfg);
+    if (avail < w.device + (cfg->band_mode == GWB200_POA_FULL_BAND ? 0 : w.matrix) || w.device + w.matrix <= 0)
     {
-        std::string msg = "Requires at least " + std::to_string(sz.dev_per_poa + sz.dev_per_matrix) +
-                          " bytes of device memory per CUDAPOA batch to process correctly.";
-        delete b;
+        std::string msg = "Requires at least " + std::to_string(w.device + w.matrix) + " bytes of device memory per CUDAPOA batch to process correctly.";
         return set_error(GWB200_E_RUNTIME, msg.c_str());
     }
-    int64_t max_poas = avail / (sz.dev_per_poa + sz.dev_per_matrix);
-    max_poas         = std::max<int64_t>(1, std::min<int64_t>(max_poas, 1 << 20));
-    b->max_poas      = static_cast<int32_t>(max_poas);
-    const int64_t n  = max_poas;
-    const int64_t mn = cfg->max_nodes_per_graph;
-    const int64_t mc = cfg->max_consensus_size;
+    const int64_t n = std::max<int64_t>(1, std::min<int64_t>(avail / (w.device + w.matrix), 1 << 20));
+    b->max_poas     = static_cast<int32_t>(n);
 
-    // ---- pinned host block
+    Arena h{nullptr, n}, d{nullptr, n};
+    const int64_t total_h = n * w.host + kHostReserve;
+    if (!b->h_block.ensure(total_h))
+        return set_error(GWB200_E_BAD_ALLOC, "pinned host allocation failed");
+    h.base                = b->h_block.p;
+    const int64_t total_d = n * (w.device + w.matrix) + kDeviceReserve;
+    if (ext_block)
     {
-        int64_t total_h = n * sz.host_per_poa + 4096 * 2 + 4096;
-        if (!b->h_block.ensure(total_h))
+        if (total_d > ext_bytes)
         {
-            delete b;
-            return set_error(GWB200_E_BAD_ALLOC, "pinned host allocation failed");
+            std::string msg = "Requires at least " + std::to_string(total_d) + " bytes of device memory per CUDAPOA batch to process correctly.";
+            return set_error(GWB200_E_RUNTIME, msg.c_str());
         }
-        Carver hc{b->h_block.p};
-        b->seq_capacity  = n * sz.seq_bytes_per_poa;
-        b->h_sequences   = hc.take<uint8_t>(b->seq_capacity + 4096);
-        b->h_weights     = hc.take<int8_t>(b->seq_capacity + 4096);
-        b->h_seq_lengths = hc.take<int32_t>(n * cfg->max_sequences_per_poa);
-        b->h_windows     = hc.take<WindowInfo>(n);
-        b->h_consensus   = hc.take<uint8_t>(n * mc);
-        b->h_coverage    = hc.take<uint16_t>(n * mc);
-        b->h_cons_len    = hc.take<int32_t>(n);
-        b->h_status      = hc.take<int32_t>(n);
-        b->h_node_count  = hc.take<int32_t>(n);
-        b->h_cells       = hc.take<unsigned long long>(n);
-        if (b->msa)
-            b->h_msa = hc.take<uint8_t>(n * cfg->max_sequences_per_poa * mc);
-        if (hc.off > total_h + 256 * 16)
-        {
-            // host_per_poa has 64 B slack per POA; the 256 B carve alignment of 12 arrays is covered by the constant above
-        }
-        std::memset(b->h_sequences, 0, b->seq_capacity + 4096);
+        d.base = static_cast<uint8_t*>(ext_block);
     }
-    // ---- device block
+    else
     {
-        const int64_t fixed   = fixed_dev;
-        const int64_t total_d = n * (sz.dev_per_poa + sz.dev_per_matrix) + fixed;
-        if (ext_block)
-        {
-            if (total_d > ext_bytes)
-            {
-                std::string msg = "Requires at least " + std::to_string(total_d) + " bytes of device memory per CUDAPOA batch to process correctly.";
-                delete b;
-                return set_error(GWB200_E_RUNTIME, msg.c_str());
-            }
-            b->d_block     = static_cast<uint8_t*>(ext_block);
-            b->owns_dblock = false;
-        }
-        else if (cudaMalloc(reinterpret_cast<void**>(&b->d_block), total_d) != cudaSuccess)
+        if (cudaMalloc(reinterpret_cast<void**>(&d.base), total_d) != cudaSuccess)
         {
             cudaGetLastError();
-            delete b;
             return set_error(GWB200_E_BAD_ALLOC, "Out of memory: device allocation for the POA batch failed");
         }
-        Carver dc{b->d_block};
-        DeviceParams& P = b->P;
-        const int64_t S = b->size_bytes;
-        P.sequences     = dc.take<uint8_t>(b->seq_capacity + 4096);
-        P.weights       = dc.take<int8_t>(b->seq_capacity + 4096);
-        P.seq_lengths   = dc.take<int32_t>(n * cfg->max_sequences_per_poa);
-        P.windows       = dc.take<WindowInfo>(n);
-        P.nodes         = dc.take<uint8_t>(n * mn);
-        P.in_cnt        = dc.take<uint16_t>(n * mn);
-        P.out_cnt       = dc.take<uint16_t>(n * mn);
-        P.aln_cnt       = dc.take<uint16_t>(n * mn);
-        P.node_cov      = dc.take<uint16_t>(n * mn);
-        P.local_cnt     = dc.take<uint16_t>(n * mn);
-        P.in_edges      = dc.take<uint8_t>(n * mn * kMaxEdges * S);
-        P.out_edges     = dc.take<uint8_t>(n * mn * kMaxEdges * S);
-        P.aligned       = dc.take<uint8_t>(n * mn * kMaxAligned * S);
-        P.in_w          = dc.take<uint16_t>(n * mn * kMaxEdges);
-        P.sorted        = dc.take<uint8_t>(n * mn * S);
-        P.pos           = dc.take<uint8_t>(n * mn * S);
-        P.aln_graph     = dc.take<uint8_t>(n * sz.aln_capacity * S);
-        P.aln_read      = dc.take<uint8_t>(n * sz.aln_capacity * S);
-        P.cons_scores   = dc.take<int32_t>(n * mn);
-        P.cons_preds    = dc.take<uint8_t>(n * mn * S);
-        P.consensus     = dc.take<uint8_t>(n * mc);
-        P.coverage      = dc.take<uint16_t>(n * mc);
-        P.consensus_len = dc.take<int32_t>(n);
-        P.status        = dc.take<int32_t>(n);
-        P.node_count    = dc.take<int32_t>(n);
-        P.cells         = dc.take<unsigned long long>(n);
-        if (b->msa)
-        {
-            P.seq_path       = dc.take<uint8_t>((b->seq_capacity + 4096) * S);
-            P.msa_col        = dc.take<uint8_t>(n * mn * S);
-            P.marks          = dc.take<uint8_t>(n * mn);
-            P.check          = dc.take<uint8_t>(n * mn);
-            P.stack          = dc.take<uint8_t>(n * sz.stack_capacity * S);
-            P.stack_capacity = sz.stack_capacity;
-            P.msa_out        = dc.take<uint8_t>(n * cfg->max_sequences_per_poa * mc);
-        }
-        else if (b->accurate)
-        {
-            P.marks          = dc.take<uint8_t>(n * mn);
-            P.check          = dc.take<uint8_t>(n * mn);
-            P.stack          = dc.take<uint8_t>(n * sz.stack_capacity * S);
-            P.stack_capacity = sz.stack_capacity;
-        }
-        b->X.row_meta    = dc.take<int4>(n * (mn + 1));
-        b->X.rd_capacity = align_up(std::max(cfg->max_sequence_size, 1), 4) + 8;
-        b->X.rd_node     = dc.take<uint8_t>(n * static_cast<int64_t>(b->X.rd_capacity) * S);
-        b->d_timers      = dc.take<unsigned long long>(n * 8);
-        b->X.work_counter = dc.take<int32_t>(64);
-        b->X.timers      = nullptr;
-        b->X.tb_scores   = nullptr;
-        b->X.tb_trace    = nullptr;
-        b->X.tb_height   = cfg->max_banded_pred_distance;
-        b->X.tb_trace16  = b->trace_bytes == 2 ? 1 : 0;
-        if (b->tb_mode)
-            b->X.tb_scores = dc.take<uint8_t>(n * (static_cast<int64_t>(cfg->matrix_sequence_dimension) * cfg->max_banded_pred_distance * b->score_bytes + 256));
-        // everything that is left is the score pool (allocate_block.hpp:227-239)
-        dc.off                 = align_up64(dc.off, 256);
-        P.scores               = b->d_block + dc.off;
-        b->scorebuf_alloc_size = total_d - dc.off;
-        if (b->tb_mode)
-        {
-            // in the traceback modes the pooled remainder is the trace matrix (allocate_block.hpp:236-239); cells the walk may
-            // read without a prior write (row 0, unreachable boundary cells) are defined as zero
-            b->X.tb_trace = P.scores;
-            cudaMemsetAsync(P.scores, 0, b->scorebuf_alloc_size, b->stream);
-        }
-        P.max_nodes            = cfg->max_nodes_per_graph;
-        P.matrix_seq_dim       = cfg->matrix_sequence_dimension;
-        P.max_consensus        = cfg->max_consensus_size;
-        P.max_seqs             = cfg->max_sequences_per_poa;
-        P.band_width           = cfg->alignment_band_width;
-        P.band_mode            = cfg->band_mode;
-        P.gap                  = b->gap;
-        P.mismatch             = b->mismatch;
-        P.match                = b->match;
-        P.msa                  = b->msa ? 1 : 0;
-        P.accurate             = b->accurate ? 1 : 0;
-        P.aln_capacity         = sz.aln_capacity;
+        b->d_block.reset(d.base);
     }
-    if (b->kernel == PoaKernel::v3)
-        b->X.pool_bytes = v3_pool_bytes(b);
-    else if (b->kernel == PoaKernel::tb)
-        b->X.pool_bytes = tb_pool_bytes(b);
-    else
-        b->X.pool_bytes = kV1PoolBytes;
-    gwb200_poa_batch_reset(b);
-    *out = b;
+    lay_out(h, d, b->shape, *cfg, *b);
+    d.off = align_up64(d.off, 256);
+    if (h.off > total_h || d.off > total_d)
+        return set_error(GWB200_E_RUNTIME, "the POA batch's arrays outgrew the blocks sized for them");
+    std::memset(b->h_sequences, 0, n * window_bases(*cfg) + kSeqTail);
+
+    // everything that is left of the device block is the score pool (allocate_block.hpp:227-239)
+    DeviceParams& P        = b->P;
+    P.scores               = d.base + d.off;
+    b->scorebuf_alloc_size = total_d - d.off;
+    b->X.tb_height         = cfg->max_banded_pred_distance;
+    b->X.tb_trace16        = b->shape.trace_bytes == 2 ? 1 : 0;
+    if (b->shape.tb)
+    {
+        // in the traceback modes the pooled remainder is the trace matrix (allocate_block.hpp:236-239); cells the walk may
+        // read without a prior write (row 0, unreachable boundary cells) are defined as zero
+        b->X.tb_trace = P.scores;
+        cudaMemsetAsync(P.scores, 0, b->scorebuf_alloc_size, b->stream);
+    }
+    P.max_nodes      = cfg->max_nodes_per_graph;
+    P.matrix_seq_dim = cfg->matrix_sequence_dimension;
+    P.max_consensus  = cfg->max_consensus_size;
+    P.max_seqs       = cfg->max_sequences_per_poa;
+    P.band_width     = cfg->alignment_band_width;
+    P.band_mode      = cfg->band_mode;
+    P.gap            = b->gap;
+    P.mismatch       = b->mismatch;
+    P.match          = b->match;
+    P.msa            = b->shape.msa ? 1 : 0;
+    P.accurate       = b->shape.accurate ? 1 : 0;
+    b->X.pool_bytes  = pool_bytes(b.get());
+    gwb200_poa_batch_reset(b.get());
+    *out = b.release();
     return 0;
 }
 
@@ -722,8 +692,6 @@ void gwb200_poa_batch_destroy(gwb200_poa_batch* b)
         return;
     DeviceGuard guard(b->device_id);
     cudaStreamSynchronize(b->stream);
-    if (b->d_block && b->owns_dblock)
-        cudaFree(b->d_block);
     delete b;
 }
 
@@ -759,7 +727,7 @@ int gwb200_poa_batch_add_group(gwb200_poa_batch* b, int32_t n, const char* const
     // reserve_buf
     {
         const int64_t width = (c.band_mode != GWB200_POA_FULL_BAND) ? c.matrix_sequence_dimension : align_up(max_seq_length + 1 + kCPT, 4);
-        const int64_t req   = width * static_cast<int64_t>(c.max_nodes_per_graph) * (b->tb_mode ? b->trace_bytes : b->score_bytes); // cudapoa_batch.cuh:551-553
+        const int64_t req   = width * static_cast<int64_t>(c.max_nodes_per_graph) * (b->shape.tb ? b->shape.trace_bytes : b->shape.score_bytes); // cudapoa_batch.cuh:551-553
         if (req > b->avail_buf_mem)
             return GWB200_POA_EXCEEDED_MAXIMUM_POAS;
         b->avail_buf_mem -= req;
@@ -932,12 +900,12 @@ int gwb200_poa_batch_add_groups_flat(gwb200_poa_batch* b, int32_t n_windows, con
 int32_t gwb200_poa_batch_total_poas(const gwb200_poa_batch* b) { return b ? b->poa_count : 0; }
 int32_t gwb200_poa_batch_max_poas(const gwb200_poa_batch* b) { return b ? b->max_poas : 0; }
 int32_t gwb200_poa_batch_id(const gwb200_poa_batch* b) { return b ? b->bid : -1; }
-int32_t gwb200_poa_batch_score_bytes(const gwb200_poa_batch* b) { return b ? b->score_bytes : 0; }
+int32_t gwb200_poa_batch_score_bytes(const gwb200_poa_batch* b) { return b ? b->shape.score_bytes : 0; }
 int32_t gwb200_poa_batch_kernel(const gwb200_poa_batch* b)
 {
     if (!b)
         return -1;
-    return b->kernel == PoaKernel::tb ? 0 : (b->kernel == PoaKernel::v3 ? 1 : 2);
+    return b->shape.kernel == PoaKernel::tb ? 0 : (b->shape.kernel == PoaKernel::v3 ? 1 : 2);
 }
 int32_t gwb200_poa_batch_pool_bytes(const gwb200_poa_batch* b) { return b ? b->X.pool_bytes : 0; }
 
@@ -968,7 +936,21 @@ int gwb200_poa_batch_launch(gwb200_poa_batch* b)
     DeviceGuard guard(b->device_id);
     b->P.n_windows = b->poa_count;
     GWB200_CUDA_TRY(b->timer.record_start(b->stream));
-    batch_action(b, 0);
+    const WindowKernel kfn = window_kernel(b);
+    const int32_t nb       = resident_ctas(b, kfn);
+    b->X.timers            = b->timers_on ? b->d_timers : nullptr;
+    if (b->timers_on)
+        cudaMemsetAsync(b->d_timers, 0, sizeof(unsigned long long) * 8 * b->poa_count, b->stream);
+    int32_t grid = b->poa_count;
+    if (b->shape.kernel == PoaKernel::v3)
+    {
+        int sms = 132;
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, b->device_id);
+        grid = std::max(1, std::min(b->poa_count, std::max(1, nb) * sms));
+        cudaMemsetAsync(b->X.work_counter, 0, sizeof(int32_t), b->stream);
+    }
+    kfn<<<grid, 32, b->X.pool_bytes, b->stream>>>(b->P, b->X);
+    count_launch();
     GWB200_CUDA_TRY(cudaPeekAtLastError());
     GWB200_CUDA_TRY(b->timer.record_stop(b->stream));
     b->launched        = true;
@@ -1108,7 +1090,7 @@ int gwb200_poa_batch_get_graphs(gwb200_poa_batch* b, int32_t* node_counts, int32
         GWB200_CUDA_TRY(cudaMemcpy(nodes.data(), b->P.nodes, n * mn, cudaMemcpyDeviceToHost));
     }
     int64_t node_off = 0, edge_off = 0;
-    std::vector<uint8_t> ebuf(mn * b->size_bytes);
+    std::vector<uint8_t> ebuf(mn * b->shape.size_bytes);
     std::vector<uint16_t> wbuf(mn);
     for (int64_t w = 0; w < n; w++)
     {
@@ -1136,15 +1118,15 @@ int gwb200_poa_batch_get_graphs(gwb200_poa_batch* b, int32_t* node_counts, int32
                 first[i + 1] = first[i] + in_cnt[w * mn + i];
             for (int32_t slot = 0; slot < max_in; slot++)
             {
-                const uint8_t* dsrc = static_cast<const uint8_t*>(b->P.in_edges) + (w * mn * kMaxEdges + slot * mn) * b->size_bytes;
-                GWB200_CUDA_TRY(cudaMemcpy(ebuf.data(), dsrc, nc * b->size_bytes, cudaMemcpyDeviceToHost));
+                const uint8_t* dsrc = static_cast<const uint8_t*>(b->P.in_edges) + (w * mn * kMaxEdges + slot * mn) * b->shape.size_bytes;
+                GWB200_CUDA_TRY(cudaMemcpy(ebuf.data(), dsrc, nc * b->shape.size_bytes, cudaMemcpyDeviceToHost));
                 GWB200_CUDA_TRY(cudaMemcpy(wbuf.data(), b->P.in_w + w * mn * kMaxEdges + slot * mn, nc * 2, cudaMemcpyDeviceToHost));
                 for (int32_t i = 0; i < nc; i++)
                 {
                     if (slot < in_cnt[w * mn + i])
                     {
                         const int64_t k = edge_off + first[i] + slot;
-                        edge_src[k]     = b->size_bytes == 2 ? reinterpret_cast<int16_t*>(ebuf.data())[i] : reinterpret_cast<int32_t*>(ebuf.data())[i];
+                        edge_src[k]     = b->shape.size_bytes == 2 ? reinterpret_cast<int16_t*>(ebuf.data())[i] : reinterpret_cast<int32_t*>(ebuf.data())[i];
                         edge_dst[k]     = i;
                         edge_weight[k]  = wbuf[i];
                     }
@@ -1189,7 +1171,7 @@ int32_t gwb200_poa_batch_resident_windows(gwb200_poa_batch* b)
     DeviceGuard guard(b->device_id);
     int sms = 0;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, b->device_id);
-    return sms * batch_action(b, 1);
+    return sms * resident_ctas(b, window_kernel(b));
 }
 
 int gwb200_poa_batch_enable_timers(gwb200_poa_batch* b, int32_t on)
@@ -1222,18 +1204,18 @@ int gwb200_device_fdividef(int32_t n, const float* a, const float* b, float* out
 {
     if (n <= 0)
         return 0;
-    float *da = nullptr, *db = nullptr, *dout = nullptr;
-    GWB200_CUDA_TRY(cudaMalloc(&da, 4 * n));
-    GWB200_CUDA_TRY(cudaMalloc(&db, 4 * n));
-    GWB200_CUDA_TRY(cudaMalloc(&dout, 4 * n));
-    GWB200_CUDA_TRY(cudaMemcpy(da, a, 4 * n, cudaMemcpyHostToDevice));
-    GWB200_CUDA_TRY(cudaMemcpy(db, b, 4 * n, cudaMemcpyHostToDevice));
-    fdividef_kernel<<<(n + 255) / 256, 256>>>(n, da, db, dout);
+    std::unique_ptr<float, CudaFree> da, db, dout;
+    for (auto* d : {&da, &db, &dout})
+    {
+        float* p = nullptr;
+        GWB200_CUDA_TRY(cudaMalloc(&p, 4 * n));
+        d->reset(p);
+    }
+    GWB200_CUDA_TRY(cudaMemcpy(da.get(), a, 4 * n, cudaMemcpyHostToDevice));
+    GWB200_CUDA_TRY(cudaMemcpy(db.get(), b, 4 * n, cudaMemcpyHostToDevice));
+    fdividef_kernel<<<(n + 255) / 256, 256>>>(n, da.get(), db.get(), dout.get());
     count_launch();
-    GWB200_CUDA_TRY(cudaMemcpy(out, dout, 4 * n, cudaMemcpyDeviceToHost));
-    cudaFree(da);
-    cudaFree(db);
-    cudaFree(dout);
+    GWB200_CUDA_TRY(cudaMemcpy(out, dout.get(), 4 * n, cudaMemcpyDeviceToHost));
     return 0;
 }
 
