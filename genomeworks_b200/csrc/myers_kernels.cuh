@@ -20,6 +20,7 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "async_copy.cuh"
 #include "myers_skew.cuh"
 
 namespace gwb200
@@ -81,40 +82,12 @@ struct DeviceParams
 
 __device__ __forceinline__ int32_t ceil_div(int32_t a, int32_t b) { return (a + b - 1) / b; }
 
-// ---- shared-memory / TMA helpers (1-D bulk asynchronous copy completing on an mbarrier)
-__device__ __forceinline__ uint32_t smem_addr(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
+// 32-bit load from a shared-memory address (smem_addr, async_copy.cuh)
 __device__ __forceinline__ uint32_t lds_u32(uint32_t a)
 {
     uint32_t v;
     asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a));
     return v;
-}
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, uint32_t count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(unsigned long long* bar, uint32_t bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_load_g2s(void* sdst, const void* gsrc, uint32_t bytes, unsigned long long* bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_addr(sdst)),
-                 "l"(__cvta_generic_to_global(gsrc)), "r"(bytes), "r"(smem_addr(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t parity)
-{
-    uint32_t done = 0, spins = 0;
-    while (!done)
-    {
-        asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}\n"
-                     : "=r"(done)
-                     : "r"(smem_addr(bar)), "r"(parity)
-                     : "memory");
-        if (++spins > (1u << 22))
-            __trap(); // a copy that never completes is a bug: fail loudly instead of hanging the device
-    }
 }
 
 // Query bit patterns of the fast path: [4][n_words + 1] words in shared memory (one zero word of padding per character, so the

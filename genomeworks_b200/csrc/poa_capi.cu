@@ -137,7 +137,7 @@ struct PoaArrays
     uint8_t* h_msa              = nullptr;
 
     DeviceParams P{};
-    V2Extra X{};
+    ExtraParams X{};
     unsigned long long* d_timers = nullptr;
 };
 
@@ -154,7 +154,7 @@ void lay_out(Arena& h, Arena& d, const BatchShape& s, const gwb200_poa_config& c
     const int64_t mn = c.max_nodes_per_graph, mc = c.max_consensus_size, ms = c.max_sequences_per_poa, S = s.size_bytes;
     const int64_t bases = window_bases(c);
     DeviceParams& P     = a.P;
-    V2Extra& X          = a.X;
+    ExtraParams& X      = a.X;
     P.aln_capacity      = c.max_nodes_per_graph + c.max_sequence_size + 16;
     P.stack_capacity    = (s.msa || s.accurate) ? 4 * c.max_nodes_per_graph + 16 : 0;
     X.rd_capacity       = align_up(std::max(c.max_sequence_size, 1), 4) + 8;
@@ -333,7 +333,7 @@ int32_t pool_bytes(const gwb200_poa_batch* b)
     }
 }
 
-using WindowKernel = void (*)(const DeviceParams, const V2Extra);
+using WindowKernel = void (*)(const DeviceParams, const ExtraParams);
 
 template <typename ScoreT, typename SizeT>
 WindowKernel typed_kernel(PoaKernel k)

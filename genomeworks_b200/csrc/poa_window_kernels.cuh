@@ -1,17 +1,21 @@
 // gw-b200 POA window kernels (sm_90a): one per-window pipeline, three alignment steps.
 //
 // process_window runs one window on one warp, from the backbone to the consensus / MSA (cudapoa_kernels.cuh:200-541): backbone
-// from read 0, then per read the alignment, the graph update (add_alignment_v2) and the topological sort (topsort_v3, or racon's
-// sort under SPOA_ACCURATE), then the consensus or the MSA. The kernels differ only in the alignment step they pass in:
-//   poa_window_kernel_v3  nw_banded_v3 (or nw_full for the full band); persistent grid, every band up to the widest adaptive band
-//   poa_window_kernel_tb  nw_banded_tb; one window per CTA, the traceback band modes
-//   poa_window_kernel     nw_banded (or nw_full); one window per CTA, wider static bands and reads of 64 k bases and more
+// from read 0, then per read the alignment, the graph update (add_alignment) and the topological sort (topsort, or racon's
+// sort under SPOA_ACCURATE), then the consensus or the MSA (poa_graph.cuh). The kernels differ only in the alignment step they
+// pass in:
+//   poa_window_kernel_v3  nw_banded_v3 (poa_nw_v3.cuh) or nw_full for the full band; persistent grid, every band up to the widest
+//                         adaptive band
+//   poa_window_kernel_tb  nw_banded_tb (poa_nw_tb.cuh); one window per CTA, the traceback band modes
+//   poa_window_kernel     nw_banded or nw_full (poa_nw.cuh); one window per CTA, wider static bands and reads of 64 k bases and more
 #pragma once
 
-#include "poa_kernels.cuh"
-#include "poa_kernels_tb.cuh"
-#include "poa_kernels_v2.cuh"
-#include "poa_kernels_v3.cuh"
+#include "async_copy.cuh"
+#include "poa_common.cuh"
+#include "poa_graph.cuh"
+#include "poa_nw.cuh"
+#include "poa_nw_tb.cuh"
+#include "poa_nw_v3.cuh"
 
 namespace gwb200
 {
@@ -41,7 +45,7 @@ __device__ __forceinline__ int32_t align_with_rerun(const bool adaptive, Nw nw)
 // code counts as an empty alignment). scores is window w's score matrix, matrix_size the elements of a banded one (of the trace
 // matrix in the traceback modes), row_meta the window's row records (v3).
 template <typename ScoreT, typename SizeT, typename Align>
-__device__ void process_window(const DeviceParams& P, const V2Extra& X, const int32_t w, uint8_t* pool, Align align)
+__device__ void process_window(const DeviceParams& P, const ExtraParams& X, const int32_t w, uint8_t* pool, Align align)
 {
     const bool MSA      = P.msa != 0;
     const int32_t lane  = threadIdx.x & 31;
@@ -160,7 +164,7 @@ __device__ void process_window(const DeviceParams& P, const V2Extra& X, const in
             {
                 unsigned long long t_ph__ = timers ? clock64() : 0ull;
                 int32_t nc = node_count;
-                error      = add_alignment_v2<SizeT>(g, nc, alen, aln_graph, sequence, seq_len, aln_read, base_weights, path, rd_node);
+                error      = add_alignment<SizeT>(g, nc, alen, aln_graph, sequence, seq_len, aln_read, base_weights, path, rd_node);
                 GWB200_TIMER_LAP(3);
                 if (!error)
                 {
@@ -173,7 +177,7 @@ __device__ void process_window(const DeviceParams& P, const V2Extra& X, const in
                     }
                     else
                     {
-                        topsort_v3<SizeT>(g, nc, pool, X.pool_bytes, row_meta); // no alignment step reads row_meta across reads
+                        topsort<SizeT>(g, nc, pool, X.pool_bytes, row_meta); // no alignment step reads row_meta across reads
                     }
                 }
                 GWB200_TIMER_LAP(4);
@@ -219,7 +223,7 @@ __device__ void process_window(const DeviceParams& P, const V2Extra& X, const in
 
 // Persistent grid: one warp per CTA, every CTA pulls window indices from the batch's work counter until none is left.
 template <typename ScoreT, typename SizeT>
-__global__ void __launch_bounds__(32, (sizeof(ScoreT) == 4 ? 12 : 16)) poa_window_kernel_v3(const DeviceParams P, const V2Extra X)
+__global__ void __launch_bounds__(32, (sizeof(ScoreT) == 4 ? 12 : 16)) poa_window_kernel_v3(const DeviceParams P, const ExtraParams X)
 {
     extern __shared__ __align__(16) uint8_t pool[];
     __shared__ __align__(16) V3Shared sh;
@@ -262,7 +266,7 @@ __global__ void __launch_bounds__(32, (sizeof(ScoreT) == 4 ? 12 : 16)) poa_windo
 
 // One window per CTA of one warp: the traceback band modes (trace matrix in the pooled buffer, score ring in X.tb_scores).
 template <typename ScoreT, typename SizeT>
-__global__ void __launch_bounds__(32, 16) poa_window_kernel_tb(const DeviceParams P, const V2Extra X)
+__global__ void __launch_bounds__(32, 16) poa_window_kernel_tb(const DeviceParams P, const ExtraParams X)
 {
     extern __shared__ __align__(16) uint8_t pool[];
     if (blockIdx.x >= P.n_windows)
@@ -289,7 +293,7 @@ __global__ void __launch_bounds__(32, 16) poa_window_kernel_tb(const DeviceParam
 // CTAs per SM, five warps in each quarter of the register file: at most 96 registers, as many windows per SM as the kernel had when
 // its graph update and sort were serial (with 16 CTAs a batch of 2 133 windows at static band 2048 needs two waves).
 template <typename ScoreT, typename SizeT>
-__global__ void __launch_bounds__(32, 20) poa_window_kernel(const DeviceParams P, const V2Extra X)
+__global__ void __launch_bounds__(32, 20) poa_window_kernel(const DeviceParams P, const ExtraParams X)
 {
     extern __shared__ __align__(16) uint8_t pool[];
     if (blockIdx.x >= P.n_windows)
@@ -317,6 +321,14 @@ __global__ void __launch_bounds__(32, 20) poa_window_kernel(const DeviceParams P
         });
     };
     process_window<ScoreT, SizeT>(P, X, blockIdx.x, pool, align);
+}
+
+// __fdividef on the device (gwb200_device_fdividef), so that the CPU oracle can place bands with the division of band_gradient
+__global__ void fdividef_kernel(int32_t n, const float* a, const float* b, float* out)
+{
+    int32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n)
+        out[i] = __fdividef(a[i], b[i]);
 }
 
 } // namespace poa

@@ -239,7 +239,7 @@ def test_static_band_512_and_128_vs_reference():
 
 
 def test_static_band_2048_first_generation_kernel_vs_oracle(device_fdiv):
-    """A band wider than the widest adaptive band (1536) runs the first-generation kernel (poa_kernels.cuh)."""
+    """A band wider than the widest adaptive band (1536) runs the first-generation kernel (nw_banded, poa_nw.cuh)."""
     from genomeworks_b200 import cudapoa, synth
     win_nseq, seq_len, data = synth.poa_windows(24, 900, 10, 10, 5, 5, seed0=2048, max_read_len=1024)
     cfg = cudapoa.make_config(1024, 16, 2048, "static_band")

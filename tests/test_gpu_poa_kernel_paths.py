@@ -1,6 +1,6 @@
 """The POA kernels on the code paths their config and inputs select, against the CPU oracle.
 
-v3 (poa_kernels_v3.cuh) runs every non-traceback batch with a band of at most 1536 and reads shorter than 65 536 bases. Its DP
+v3 (poa_nw_v3.cuh) runs every non-traceback batch with a band of at most 1536 and reads shorter than 65 536 bases. Its DP
 rows take different code depending on:
   - the chunks per row, ceil(band / 256) (int16 rows in groups of two chunks, int32 rows one at a time, a half chunk at the end);
   - the depth R of the shared-memory ring of score rows, min(pool_bytes / row_bytes, 64), where the pool per CTA shrinks as more
@@ -125,7 +125,7 @@ def flat(windows):
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
-# the adaptive band of nw_banded_v3 (poa_kernels_v3.cuh, before the rows) and the ring depth of dp_rows_v3
+# the adaptive band of nw_banded_v3 (widen_band and set_band in poa_common.cuh) and the ring depth of dp_rows_v3
 # ---------------------------------------------------------------------------------------------------------------------------
 
 
