@@ -254,8 +254,8 @@ struct gwb200_poa_batch : PoaArrays
 
     int32_t max_poas = 0;
     int32_t poa_count = 0;
-    int32_t num_nucleotides_copied = 0;
-    int32_t global_sequence_idx = 0;
+    int64_t num_nucleotides_copied = 0; // a batch may stage more than 2^31 bases and reads
+    int64_t global_sequence_idx = 0;
     int64_t avail_buf_mem = 0, scorebuf_alloc_size = 0;
     int64_t next_scores_offset = 0;
 

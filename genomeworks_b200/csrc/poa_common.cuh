@@ -55,15 +55,17 @@ enum BandMode : int32_t
     bm_adaptive_band_traceback
 };
 
-// Host-packed description of one window (cf. WindowDetails, cudapoa_structs.cuh:70-87).
+// Host-packed description of one window (cf. WindowDetails, cudapoa_structs.cuh:70-87). The offsets are 64-bit: a batch may hold
+// more than 2^31 bases or reads.
 struct WindowInfo
 {
     int32_t num_seqs;
-    int32_t seq_len_offset; // first entry in seq_lengths
-    int32_t seq_start;      // first byte in sequences / weights / seq_path (4-byte aligned; every read is padded to 4)
     int32_t scores_width;   // full_band only: row stride of this window's score matrix
+    int64_t seq_len_offset; // first entry in seq_lengths
+    int64_t seq_start;      // first byte in sequences / weights, first entry in seq_path (4-byte aligned; every read is padded to 4)
     int64_t scores_offset;  // full_band only: element offset / max_nodes (as in the reference)
 };
+static_assert(sizeof(WindowInfo) == 32, "WindowInfo: two int32_t then three int64_t, no padding");
 
 struct DeviceParams
 {
