@@ -175,153 +175,143 @@ def lib():
     L.gwb200_poa_batch_enable_timers.argtypes = [C.c_void_p, C.c_int32]
     L.gwb200_poa_batch_get_timers.argtypes = [C.c_void_p, C.c_void_p]
     L.gwb200_device_fdividef.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-    if hasattr(L, "gwb200_aligner_create"):
-        L.gwb200_aligner_create.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.c_int32, C.c_int64]
-        L.gwb200_aligner_destroy.argtypes = [C.c_void_p]
-        L.gwb200_aligner_destroy.restype = None
-        L.gwb200_aligner_add_alignment.argtypes = [C.c_void_p, C.c_int32, C.c_char_p, C.c_int32, C.c_char_p, C.c_int32, C.c_int32, C.c_int32]
-        for name in ("align_all", "sync_alignments", "num_alignments", "reset", "free_temporary_device_buffers"):
-            getattr(L, "gwb200_aligner_" + name).argtypes = [C.c_void_p]
-        L.gwb200_aligner_reset_max_bandwidth.argtypes = [C.c_void_p, C.c_int32]
-        L.gwb200_aligner_result_info.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
-        L.gwb200_aligner_result_runs.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
-        L.gwb200_aligner_last_cells.argtypes = [C.c_void_p]
-        L.gwb200_aligner_last_cells.restype = C.c_int64
-        L.gwb200_aligner_last_kernel_ms.argtypes = [C.c_void_p]
-        L.gwb200_aligner_last_kernel_ms.restype = C.c_float
-        L.gwb200_aligner_last_launch_info.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
-        L.gwb200_aligner_create_with_allocator.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p,
-                                                           C.c_void_p, C.c_void_p]
-    if hasattr(L, "gwb200_aligner_add_alignments"):
-        L.gwb200_aligner_add_alignments.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]
-        L.gwb200_aligner_results_flat.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
-    if hasattr(L, "gwb200_global_aligner_create"):
-        L.gwb200_global_aligner_create.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
-                                                   C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gwb200_global_aligner_destroy.argtypes = [C.c_void_p]
-        L.gwb200_global_aligner_destroy.restype = None
-        L.gwb200_global_aligner_add_alignment.argtypes = [C.c_void_p, C.c_char_p, C.c_int32, C.c_char_p, C.c_int32, C.c_int32, C.c_int32]
-        for name in ("align_all", "sync_alignments", "num_alignments", "reset"):
-            getattr(L, "gwb200_global_aligner_" + name).argtypes = [C.c_void_p]
-        L.gwb200_global_aligner_result_info.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
-        L.gwb200_global_aligner_result_states.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
-        L.gwb200_global_aligner_last_cells.argtypes = [C.c_void_p]
-        L.gwb200_global_aligner_last_cells.restype = C.c_int64
-        L.gwb200_global_aligner_last_kernel_ms.argtypes = [C.c_void_p]
-        L.gwb200_global_aligner_last_kernel_ms.restype = C.c_float
-    if hasattr(L, "gwb200_extender_create"):
-        L.gwb200_extender_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32]
-        L.gwb200_extender_create_with_allocator.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
-                                                            C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gwb200_extender_destroy.argtypes = [C.c_void_p]
-        L.gwb200_extender_destroy.restype = None
-        L.gwb200_extender_extend_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32]
-        L.gwb200_extender_extend_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
-                                                    C.c_void_p, C.c_void_p]
-        for name in ("sync", "num_results", "reset"):
-            getattr(L, "gwb200_extender_" + name).argtypes = [C.c_void_p]
-        L.gwb200_extender_get_results.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
-        L.gwb200_extender_last_kernel_ms.argtypes = [C.c_void_p]
-        L.gwb200_extender_last_kernel_ms.restype = C.c_float
-        L.gwb200_extender_last_positions.argtypes = [C.c_void_p]
-        L.gwb200_extender_last_positions.restype = C.c_int64
-    if hasattr(L, "gwb200_index_create"):
-        L.gwb200_index_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int64, C.c_uint32, C.c_int32, C.c_int32, C.c_int32,
-                                          C.c_double, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gwb200_index_wait.argtypes = [C.c_void_p]
-        L.gwb200_index_is_ready.argtypes = [C.c_void_p]
-        L.gwb200_index_get_arrays.argtypes = [C.c_void_p, C.POINTER(IndexArrays)]
-        L.gwb200_index_destroy.argtypes = [C.c_void_p]
-        L.gwb200_index_destroy.restype = None
-        L.gwb200_index_last_kernel_ms.argtypes = [C.c_void_p]
-        L.gwb200_index_last_kernel_ms.restype = C.c_float
-        L.gwb200_index_host_copy_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p]
-        L.gwb200_index_host_copy_finish.argtypes = [C.c_void_p]
-        L.gwb200_index_host_copy_get_arrays.argtypes = [C.c_void_p, C.POINTER(IndexArrays)]
-        L.gwb200_index_host_copy_to_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
-                                                       C.c_void_p]
-        L.gwb200_index_host_copy_destroy.argtypes = [C.c_void_p]
-        L.gwb200_index_host_copy_destroy.restype = None
-    if hasattr(L, "gwb200_matcher_create"):
-        L.gwb200_matcher_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(IndexArrays), C.POINTER(IndexArrays), C.c_void_p, C.c_int32,
-                                            C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gwb200_matcher_get_anchors.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
-        L.gwb200_matcher_copy_anchors.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
-        L.gwb200_matcher_copy_anchors.restype = C.c_int64
-        L.gwb200_matcher_key_bits.argtypes = [C.c_void_p]
-        L.gwb200_matcher_key_bits.restype = C.c_int32
-        L.gwb200_matcher_last_kernel_ms.argtypes = [C.c_void_p]
-        L.gwb200_matcher_last_kernel_ms.restype = C.c_float
-        L.gwb200_matcher_destroy.argtypes = [C.c_void_p]
-        L.gwb200_matcher_destroy.restype = None
-    if hasattr(L, "gwb200_overlapper_create"):
-        L.gwb200_overlapper_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gwb200_overlapper_get_overlaps.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_float]
-        L.gwb200_overlapper_get_overlaps.restype = C.c_int64
-        L.gwb200_overlapper_copy_overlaps.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
-        L.gwb200_overlapper_copy_overlaps.restype = C.c_int64
-        L.gwb200_overlapper_last_kernel_ms.argtypes = [C.c_void_p]
-        L.gwb200_overlapper_last_kernel_ms.restype = C.c_float
-        L.gwb200_overlapper_destroy.argtypes = [C.c_void_p]
-        L.gwb200_overlapper_destroy.restype = None
-        L.gwb200_overlaps_post_process.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64]
-        L.gwb200_overlaps_post_process.restype = C.c_int64
-    if hasattr(L, "gwb200_rescue_overlap_ends"):
-        L.gwb200_rescue_overlap_ends.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_float,
-                                                 C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gwb200_rescue_last_kernel_ms.argtypes = []
-        L.gwb200_rescue_last_kernel_ms.restype = C.c_float
-    if hasattr(L, "gwb200_mapper_create"):
-        L.gwb200_mapper_format_paf.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
-                                               C.c_int64, C.c_int32, C.c_void_p, C.c_int64]
-        L.gwb200_mapper_format_paf.restype = C.c_int64
-        L.gwb200_group_reads_into_indices.argtypes = [C.c_void_p, C.c_int64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64]
-        L.gwb200_group_reads_into_indices.restype = C.c_int64
-        L.gwb200_mapper_read_order.argtypes = [C.c_int64, C.c_void_p]
-        L.gwb200_mapper_default_params.argtypes = [C.POINTER(MapperParams)]
-        L.gwb200_mapper_default_params.restype = None
-        L.gwb200_mapper_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(MapperParams), C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32,
-                                           C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gwb200_mapper_num_tiles.argtypes = [C.c_void_p]
-        L.gwb200_mapper_num_tiles.restype = C.c_int64
-        L.gwb200_mapper_run_tile.argtypes = [C.c_void_p, C.c_int64]
-        L.gwb200_mapper_tile_results.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_void_p),
-                                                 C.POINTER(C.c_void_p)]
-        L.gwb200_mapper_align_overlaps.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32]
-        L.gwb200_mapper_index_builds.argtypes = [C.c_void_p]
-        L.gwb200_mapper_index_builds.restype = C.c_int64
-        L.gwb200_mapper_stage_ms.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
-        L.gwb200_mapper_destroy.argtypes = [C.c_void_p]
-        L.gwb200_mapper_destroy.restype = None
-    if hasattr(L, "gwb200_polisher_create"):
-        L.gwb200_polish_window_groups.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
-                                                  C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
-                                                  C.c_void_p]
-        L.gwb200_polish_window_groups_q.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
-                                                    C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_double, C.c_int32, C.c_int32,
-                                                    C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gwb200_window_groups_weights.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-        L.gwb200_correction_window_groups.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
-                                                      C.c_int64, C.c_void_p, C.c_double, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
-                                                      C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gwb200_corrector_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(PolishParams), C.c_void_p, C.c_int64, C.c_void_p, C.c_double,
-                                              C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gwb200_polisher_create_q.argtypes = [C.POINTER(C.c_void_p), C.POINTER(PolishParams), C.c_void_p, C.c_int64, C.c_void_p,
-                                               C.c_int64, C.c_void_p, C.c_double, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
-                                               C.c_void_p]
-        L.gwb200_window_groups_get.argtypes = [C.c_void_p, C.POINTER(WindowGroupsView)]
-        L.gwb200_window_groups_kernel_ms.argtypes = [C.c_void_p]
-        L.gwb200_window_groups_kernel_ms.restype = C.c_float
-        L.gwb200_window_groups_destroy.argtypes = [C.c_void_p]
-        L.gwb200_window_groups_destroy.restype = None
-        L.gwb200_polish_default_params.argtypes = [C.POINTER(PolishParams)]
-        L.gwb200_polish_default_params.restype = None
-        L.gwb200_polisher_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(PolishParams), C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
-                                             C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gwb200_polisher_run.argtypes = [C.c_void_p]
-        L.gwb200_polisher_results.argtypes = [C.c_void_p, C.POINTER(PolishResults)]
-        L.gwb200_polisher_destroy.argtypes = [C.c_void_p]
-        L.gwb200_polisher_destroy.restype = None
+    L.gwb200_aligner_create.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.c_int32, C.c_int64]
+    L.gwb200_aligner_destroy.argtypes = [C.c_void_p]
+    L.gwb200_aligner_destroy.restype = None
+    L.gwb200_aligner_add_alignment.argtypes = [C.c_void_p, C.c_int32, C.c_char_p, C.c_int32, C.c_char_p, C.c_int32, C.c_int32, C.c_int32]
+    for name in ("align_all", "sync_alignments", "num_alignments", "reset", "free_temporary_device_buffers"):
+        getattr(L, "gwb200_aligner_" + name).argtypes = [C.c_void_p]
+    L.gwb200_aligner_reset_max_bandwidth.argtypes = [C.c_void_p, C.c_int32]
+    L.gwb200_aligner_result_info.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    L.gwb200_aligner_result_runs.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    L.gwb200_aligner_last_cells.argtypes = [C.c_void_p]
+    L.gwb200_aligner_last_cells.restype = C.c_int64
+    L.gwb200_aligner_last_kernel_ms.argtypes = [C.c_void_p]
+    L.gwb200_aligner_last_kernel_ms.restype = C.c_float
+    L.gwb200_aligner_last_launch_info.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
+    L.gwb200_aligner_create_with_allocator.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p,
+                                                       C.c_void_p, C.c_void_p]
+    L.gwb200_aligner_add_alignments.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]
+    L.gwb200_aligner_results_flat.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
+    L.gwb200_global_aligner_create.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
+                                               C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_global_aligner_destroy.argtypes = [C.c_void_p]
+    L.gwb200_global_aligner_destroy.restype = None
+    L.gwb200_global_aligner_add_alignment.argtypes = [C.c_void_p, C.c_char_p, C.c_int32, C.c_char_p, C.c_int32, C.c_int32, C.c_int32]
+    for name in ("align_all", "sync_alignments", "num_alignments", "reset"):
+        getattr(L, "gwb200_global_aligner_" + name).argtypes = [C.c_void_p]
+    L.gwb200_global_aligner_result_info.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    L.gwb200_global_aligner_result_states.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
+    L.gwb200_global_aligner_last_cells.argtypes = [C.c_void_p]
+    L.gwb200_global_aligner_last_cells.restype = C.c_int64
+    L.gwb200_global_aligner_last_kernel_ms.argtypes = [C.c_void_p]
+    L.gwb200_global_aligner_last_kernel_ms.restype = C.c_float
+    L.gwb200_extender_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32]
+    L.gwb200_extender_create_with_allocator.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                                        C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_extender_destroy.argtypes = [C.c_void_p]
+    L.gwb200_extender_destroy.restype = None
+    L.gwb200_extender_extend_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32]
+    L.gwb200_extender_extend_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
+                                                C.c_void_p, C.c_void_p]
+    for name in ("sync", "num_results", "reset"):
+        getattr(L, "gwb200_extender_" + name).argtypes = [C.c_void_p]
+    L.gwb200_extender_get_results.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
+    L.gwb200_extender_last_kernel_ms.argtypes = [C.c_void_p]
+    L.gwb200_extender_last_kernel_ms.restype = C.c_float
+    L.gwb200_extender_last_positions.argtypes = [C.c_void_p]
+    L.gwb200_extender_last_positions.restype = C.c_int64
+    L.gwb200_index_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int64, C.c_uint32, C.c_int32, C.c_int32, C.c_int32,
+                                      C.c_double, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_index_wait.argtypes = [C.c_void_p]
+    L.gwb200_index_is_ready.argtypes = [C.c_void_p]
+    L.gwb200_index_get_arrays.argtypes = [C.c_void_p, C.POINTER(IndexArrays)]
+    L.gwb200_index_destroy.argtypes = [C.c_void_p]
+    L.gwb200_index_destroy.restype = None
+    L.gwb200_index_last_kernel_ms.argtypes = [C.c_void_p]
+    L.gwb200_index_last_kernel_ms.restype = C.c_float
+    L.gwb200_index_host_copy_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p]
+    L.gwb200_index_host_copy_finish.argtypes = [C.c_void_p]
+    L.gwb200_index_host_copy_get_arrays.argtypes = [C.c_void_p, C.POINTER(IndexArrays)]
+    L.gwb200_index_host_copy_to_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p]
+    L.gwb200_index_host_copy_destroy.argtypes = [C.c_void_p]
+    L.gwb200_index_host_copy_destroy.restype = None
+    L.gwb200_matcher_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(IndexArrays), C.POINTER(IndexArrays), C.c_void_p, C.c_int32,
+                                        C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_matcher_get_anchors.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
+    L.gwb200_matcher_copy_anchors.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+    L.gwb200_matcher_copy_anchors.restype = C.c_int64
+    L.gwb200_matcher_key_bits.argtypes = [C.c_void_p]
+    L.gwb200_matcher_key_bits.restype = C.c_int32
+    L.gwb200_matcher_last_kernel_ms.argtypes = [C.c_void_p]
+    L.gwb200_matcher_last_kernel_ms.restype = C.c_float
+    L.gwb200_matcher_destroy.argtypes = [C.c_void_p]
+    L.gwb200_matcher_destroy.restype = None
+    L.gwb200_overlapper_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_overlapper_get_overlaps.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_float]
+    L.gwb200_overlapper_get_overlaps.restype = C.c_int64
+    L.gwb200_overlapper_copy_overlaps.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+    L.gwb200_overlapper_copy_overlaps.restype = C.c_int64
+    L.gwb200_overlapper_last_kernel_ms.argtypes = [C.c_void_p]
+    L.gwb200_overlapper_last_kernel_ms.restype = C.c_float
+    L.gwb200_overlapper_destroy.argtypes = [C.c_void_p]
+    L.gwb200_overlapper_destroy.restype = None
+    L.gwb200_overlaps_post_process.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64]
+    L.gwb200_overlaps_post_process.restype = C.c_int64
+    L.gwb200_rescue_overlap_ends.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_float,
+                                             C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_rescue_last_kernel_ms.argtypes = []
+    L.gwb200_rescue_last_kernel_ms.restype = C.c_float
+    L.gwb200_mapper_format_paf.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                           C.c_int64, C.c_int32, C.c_void_p, C.c_int64]
+    L.gwb200_mapper_format_paf.restype = C.c_int64
+    L.gwb200_group_reads_into_indices.argtypes = [C.c_void_p, C.c_int64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64]
+    L.gwb200_group_reads_into_indices.restype = C.c_int64
+    L.gwb200_mapper_read_order.argtypes = [C.c_int64, C.c_void_p]
+    L.gwb200_mapper_default_params.argtypes = [C.POINTER(MapperParams)]
+    L.gwb200_mapper_default_params.restype = None
+    L.gwb200_mapper_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(MapperParams), C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32,
+                                       C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_mapper_num_tiles.argtypes = [C.c_void_p]
+    L.gwb200_mapper_num_tiles.restype = C.c_int64
+    L.gwb200_mapper_run_tile.argtypes = [C.c_void_p, C.c_int64]
+    L.gwb200_mapper_tile_results.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_void_p),
+                                             C.POINTER(C.c_void_p)]
+    L.gwb200_mapper_align_overlaps.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32]
+    L.gwb200_mapper_index_builds.argtypes = [C.c_void_p]
+    L.gwb200_mapper_index_builds.restype = C.c_int64
+    L.gwb200_mapper_stage_ms.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
+    L.gwb200_mapper_destroy.argtypes = [C.c_void_p]
+    L.gwb200_mapper_destroy.restype = None
+    L.gwb200_polish_window_groups.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                              C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                              C.c_void_p]
+    L.gwb200_polish_window_groups_q.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_double, C.c_int32, C.c_int32,
+                                                C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_window_groups_weights.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
+    L.gwb200_correction_window_groups.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.c_int64, C.c_void_p, C.c_double, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
+                                                  C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_corrector_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(PolishParams), C.c_void_p, C.c_int64, C.c_void_p, C.c_double,
+                                          C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_polisher_create_q.argtypes = [C.POINTER(C.c_void_p), C.POINTER(PolishParams), C.c_void_p, C.c_int64, C.c_void_p,
+                                           C.c_int64, C.c_void_p, C.c_double, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                           C.c_void_p]
+    L.gwb200_window_groups_get.argtypes = [C.c_void_p, C.POINTER(WindowGroupsView)]
+    L.gwb200_window_groups_kernel_ms.argtypes = [C.c_void_p]
+    L.gwb200_window_groups_kernel_ms.restype = C.c_float
+    L.gwb200_window_groups_destroy.argtypes = [C.c_void_p]
+    L.gwb200_window_groups_destroy.restype = None
+    L.gwb200_polish_default_params.argtypes = [C.POINTER(PolishParams)]
+    L.gwb200_polish_default_params.restype = None
+    L.gwb200_polisher_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(PolishParams), C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                         C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_polisher_run.argtypes = [C.c_void_p]
+    L.gwb200_polisher_results.argtypes = [C.c_void_p, C.POINTER(PolishResults)]
+    L.gwb200_polisher_destroy.argtypes = [C.c_void_p]
+    L.gwb200_polisher_destroy.restype = None
     _lib = L
     return L
 

@@ -2,7 +2,7 @@
 // overlap's view B is written out explicitly (its mirrored CIGAR as text, its R reverse-complemented, its qualities reversed), the
 // views are chosen per (draft, source) pair by one scan in view order, and every kept view is cut with the column walk of
 // polish_oracle.cpp and filtered as polish_quality_oracle.cpp does (both included, their entry points unchanged). TEST
-// INFRASTRUCTURE ONLY (liboracle_correct.so, built by oracle/correct.mk, bound in tests/correct_libs.py).
+// INFRASTRUCTURE ONLY (liboracle_correct.so, built by oracle/Makefile, bound in tests/correct_libs.py).
 #include "polish_quality_oracle.cpp"
 
 #include <map>

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY: a serial CPU restatement of the minimizer index (cudamapper Index), built into
-// oracle/liboracle_index.so by oracle/index.mk and loaded by tests/index_libs.py.
+// oracle/liboracle_index.so by oracle/Makefile and loaded by tests/index_libs.py.
 //
 // The contract (DESIGN.md section 10):
 //   - a read shorter than w + k - 1 bases is skipped; the others keep their own read id (first_read_id + position in the input);

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY: a serial CPU restatement of the overlapper's get_overlaps, written from DESIGN.md section 12.1 (steps
-// 1-6), built by oracle/overlapper.mk into liboracle_overlapper.so. The float division of the fraction filter is a callback, so a
+// 1-6), built by oracle/Makefile into liboracle_overlapper.so. The float division of the fraction filter is a callback, so a
 // GPU test can give it the device's __fdividef; without one it is the IEEE division.
 #include <cstdint>
 #include <cstdlib>

@@ -1,7 +1,7 @@
 // CPU restatement of the polisher's window groups (steps 2-4) and stitching (step 6), DESIGN.md section 15.1, written serially
 // from the definition and sharing no code with the library: each CIGAR is walked one column at a time, J(p) recorded for every
 // draft position of the overlap, and each window's piece cut from R. TEST INFRASTRUCTURE ONLY (liboracle_polish.so, built by
-// oracle/polish.mk, bound in tests/polish_libs.py).
+// oracle/Makefile, bound in tests/polish_libs.py).
 #include <algorithm>
 #include <cstdint>
 #include <string>

@@ -1,7 +1,7 @@
 // CPU restatement of the polisher's window groups with base qualities (steps 2-4 of DESIGN.md section 15.1 under section 15.5),
 // serial like the restatement without qualities it includes: the same CIGAR parse and column walk (polish_oracle.cpp, whose
 // entry points it leaves as they are), then each piece's weights cut from QR, the oriented qualities, and the mean-quality
-// filter applied before the depth cap. TEST INFRASTRUCTURE ONLY (liboracle_polish_q.so, built by oracle/polish_quality.mk,
+// filter applied before the depth cap. TEST INFRASTRUCTURE ONLY (liboracle_polish_q.so, built by oracle/Makefile,
 // bound in tests/polish_quality_libs.py).
 #include "polish_oracle.cpp"
 

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY -- not part of the product path.
 //
-// Thin extern "C" driver around the UNMODIFIED reference cudaextender, which oracle/extender.mk compiles from the sources
+// Thin extern "C" driver around the UNMODIFIED reference cudaextender, which oracle/Makefile compiles from the sources
 // where they lie in the reference checkout (REF=...) into oracle/_ref/libgwref_extender.so. Only tests/golden/
 // make_extender_fixture.py and tools/bench_extender.py load it. It calls nothing but the reference's public API
 // (cudaextender/include/claraparabricks/genomeworks/cudaextender/extender.hpp: create_extender + the device-pointer

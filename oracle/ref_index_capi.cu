@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY -- not part of the product path.
 //
-// Thin extern "C" driver around the UNMODIFIED reference cudamapper index, which oracle/index.mk compiles from the sources
+// Thin extern "C" driver around the UNMODIFIED reference cudamapper index, which oracle/Makefile compiles from the sources
 // where they lie in the reference checkout (REF=...) into oracle/_ref/libgwref_index.so. Only tests/golden/cudamapper/
 // make_index_fixture.py and tools/bench_index.py load it. It calls nothing but the reference's public API
 // (cudamapper/include/claraparabricks/genomeworks/cudamapper/index.hpp: Index::create_index_async + wait_to_be_ready), fed by

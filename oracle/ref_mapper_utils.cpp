@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY: C entry points over the UNMODIFIED reference's print_paf, group_reads_into_indices and kseqpp FASTA
-// parser (built by mapper.mk into _ref/libgwref_mapper_utils.so). print_paf writes to stdout; ref_print_paf captures that text.
+// parser (built by oracle/Makefile into _ref/libgwref_mapper_utils.so). print_paf writes to stdout; ref_print_paf captures that text.
 #include <claraparabricks/genomeworks/cudamapper/types.hpp>
 #include <claraparabricks/genomeworks/cudamapper/utils.hpp>
 #include <claraparabricks/genomeworks/io/fasta_parser.hpp>

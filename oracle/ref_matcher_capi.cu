@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY -- not part of the product path.
 //
-// Thin extern "C" driver around the UNMODIFIED reference cudamapper index and matcher, which oracle/matcher.mk compiles from the
+// Thin extern "C" driver around the UNMODIFIED reference cudamapper index and matcher, which oracle/Makefile compiles from the
 // sources where they lie in the reference checkout (REF=...) into oracle/_ref/libgwref_matcher.so. Only
 // tests/golden/cudamapper/make_matcher_fixture.py and tools/bench_matcher.py load it. It calls nothing but the reference's
 // public API (index.hpp: Index::create_index_async + wait_to_be_ready; matcher.hpp: Matcher::create_matcher), with an

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY -- not part of the product path.
 //
-// Thin extern "C" driver around the UNMODIFIED reference cudamapper overlapper, which oracle/overlapper.mk compiles from the
+// Thin extern "C" driver around the UNMODIFIED reference cudamapper overlapper, which oracle/Makefile compiles from the
 // sources where they lie in the reference checkout (REF=...) into oracle/_ref/libgwref_overlapper.so. Only
 // tests/golden/cudamapper/make_overlapper_fixture.py and tools/bench_overlapper.py load it. It calls nothing but the reference's
 // public API (overlapper.hpp: Overlapper::create_overlapper, get_overlaps, post_process_overlaps).

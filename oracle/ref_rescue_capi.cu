@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY -- not part of the product path.
 //
-// Thin extern "C" driver around the UNMODIFIED reference overlap-end rescue, which oracle/rescue.mk compiles from the sources
+// Thin extern "C" driver around the UNMODIFIED reference overlap-end rescue, which oracle/Makefile compiles from the sources
 // where they lie in the reference checkout (REF=...) into oracle/_ref/libgwref_rescue.so. Only
 // tests/golden/cudamapper/make_rescue_fixture.py and tools/bench_rescue.py load it. It calls nothing but the reference's public
 // API (overlapper.hpp: Overlapper::rescue_overlap_ends and details::overlapper::extend_overlap_by_sequence_similarity), through an

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY: a serial CPU restatement of the overlap-end rescue (DESIGN.md section 13.1), written from the
-// contract, for the tests to compare the engine against. Built by oracle/rescue.mk into liboracle_rescue.so.
+// contract, for the tests to compare the engine against. Built by oracle/Makefile into liboracle_rescue.so.
 //
 // Reads come flattened: read i of a set is bases[offsets[i], offsets[i + 1]). Overlaps are 36-byte cudamapper::Overlap records.
 #include <cstdint>

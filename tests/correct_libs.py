@@ -8,34 +8,23 @@ a Python restatement of view B, and the composition of read correction from prov
 - correction_case: seeded reads of a truth with each read's true segment.
 """
 import ctypes as C
-import os
 
 import numpy as np
 
 import polish_libs as pl
 import polish_quality_libs as pq
-
-ORACLE_C_PATH = os.path.join(pl.ROOT, "oracle", "liboracle_correct.so")
-
-_oracle = None
+from checker_lib import load, ptr
 
 
 def oracle():
-    global _oracle
-    if _oracle is None:
-        L = C.CDLL(ORACLE_C_PATH)
-        L.oracle_correct_groups.restype = C.c_int
-        L.oracle_correct_groups.argtypes = [C.c_void_p, C.c_int64, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_char_p,
-                                            C.c_double, C.c_int32, C.c_int32]
-        L.oracle_correct_mirror.restype = C.c_int64
-        L.oracle_correct_mirror.argtypes = [C.c_char_p, C.c_int64, C.c_uint8, C.c_char_p, C.c_int64]
-        L.oracle_correct_view.restype = C.c_int64
-        L.oracle_correct_view.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_char_p, C.c_void_p, C.c_int32, C.c_int32, C.c_char_p,
-                                          C.c_void_p]
-        L.oracle_polish_view.argtypes = [C.POINTER(pl._View)]
-        L.oracle_polish_weights.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
-        _oracle = L
-    return _oracle
+    return load("liboracle_correct.so", {
+        "oracle_correct_groups": (C.c_int, [C.c_void_p, C.c_int64, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_char_p,
+                                            C.c_double, C.c_int32, C.c_int32]),
+        "oracle_correct_mirror": (C.c_int64, [C.c_char_p, C.c_int64, C.c_uint8, C.c_char_p, C.c_int64]),
+        "oracle_correct_view": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_int64, C.c_char_p, C.c_void_p, C.c_int32, C.c_int32, C.c_char_p,
+                                            C.c_void_p]),
+        "oracle_polish_view": (C.c_int, [C.POINTER(pl._View)]),
+        "oracle_polish_weights": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)])})
 
 
 def oracle_correct_groups(overlaps, cigars, reads, window_length, max_depth, qualities=None, threshold=10.0):
@@ -48,8 +37,8 @@ def oracle_correct_groups(overlaps, cigars, reads, window_length, max_depth, qua
         qb, qoffs = pl._flat(qualities)
         assert np.array_equal(roffs, qoffs), "one quality string per read, as long as the read"
     L = oracle()
-    rc = L.oracle_correct_groups(ov.ctypes.data_as(C.c_void_p), len(ov), text, toffs.ctypes.data_as(C.c_void_p), rb,
-                                 roffs.ctypes.data_as(C.c_void_p), len(roffs) - 1, qb, threshold, window_length, max_depth)
+    rc = L.oracle_correct_groups(ptr(ov), len(ov), text, ptr(toffs), rb,
+                                 ptr(roffs), len(roffs) - 1, qb, threshold, window_length, max_depth)
     if rc != 0:
         return rc, None
     v = pl._View()
@@ -90,8 +79,8 @@ def oracle_view(overlap, cigar, reads, view, window_length):
         int(o[0]["query_end_position_in_read"] - o[0]["query_start_position_in_read"])
     rbuf = C.create_string_buffer(max(1, r_len))
     cuts = np.zeros(d_len // window_length + 3, dtype=np.int64)
-    n = oracle().oracle_correct_view(o.ctypes.data_as(C.c_void_p), c, len(c), rb, roffs.ctypes.data_as(C.c_void_p), view, window_length, rbuf,
-                                     cuts.ctypes.data_as(C.c_void_p))
+    n = oracle().oracle_correct_view(ptr(o), c, len(c), rb, ptr(roffs), view, window_length, rbuf,
+                                     ptr(cuts))
     if n < 0:
         return None
     return rbuf.raw[:r_len], cuts[:n]

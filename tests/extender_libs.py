@@ -3,17 +3,16 @@
 reference outputs tests/golden/make_extender_fixture.py stores. TEST INFRASTRUCTURE ONLY."""
 import ctypes as C
 import gzip
-import json
 import os
-import subprocess
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ORACLE_DIR = os.path.join(ROOT, "oracle")
-GOLDEN = os.path.join(ROOT, "tests", "golden", "cudaextender")
+import checker_lib
+from checker_lib import load, ptr
+
+GOLDEN = os.path.join(checker_lib.GOLDEN, "cudaextender")
 REF_OUTPUTS = os.path.join(GOLDEN, "reference_extender_outputs.json.gz")
-REF_LIB = os.path.join(ORACLE_DIR, "_ref", "libgwref_extender.so")
+REF_LIB = os.path.join(checker_lib.REF_DIR, "libgwref_extender.so")
 
 # the scoring matrix, X-drop and threshold of the reference's end-to-end test (cudaextender/tests/Test_CudaextenderEnd2End.cu)
 SAMPLE_MATRIX = np.array([91, -114, -31, -123, -1000, -1000, -100, -9100,
@@ -35,42 +34,27 @@ SIMPLE_MATRIX = SIMPLE_MATRIX.ravel()
 SEED_DTYPE = np.dtype([("query", np.uint32), ("target", np.uint32)])
 SSP_DTYPE = np.dtype([("query", np.uint32), ("target", np.uint32), ("length", np.int32), ("score", np.int32)])
 
-_oracle = None
-_ref = None
-
-
 def oracle():
-    global _oracle
-    if _oracle is None:
-        path = os.path.join(ORACLE_DIR, "liboracle_extender.so")
-        src = os.path.join(ORACLE_DIR, "extender_oracle.cpp")
-        if not os.path.exists(path) or os.path.getmtime(src) > os.path.getmtime(path):
-            subprocess.check_call(["make", "-C", ORACLE_DIR, "-f", "extender.mk", "oracle"], stdout=subprocess.DEVNULL)
-        _oracle = C.CDLL(path)
-        _oracle.oracle_extender_seed.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                                 C.c_uint32, C.c_uint32, C.c_void_p]
-        _oracle.oracle_extender_sort_unique.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
-        _oracle.oracle_extender_run.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                                C.c_void_p, C.c_int32, C.c_void_p]
-    return _oracle
-
-
-def _ptr(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return load("liboracle_extender.so", {
+        "oracle_extender_seed": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                           C.c_uint32, C.c_uint32, C.c_void_p]),
+        "oracle_extender_sort_unique": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
+        "oracle_extender_run": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                          C.c_void_p, C.c_int32, C.c_void_p])})
 
 
 def oracle_seed(query, target, matrix, xdrop, no_entropy, threshold, qs, ts):
     """-> dict(query, target, length, score, kept, total) for one seed."""
     q, t, m = np.ascontiguousarray(query, np.int8), np.ascontiguousarray(target, np.int8), np.ascontiguousarray(matrix, np.int32)
     out = np.zeros(6, dtype=np.int32)
-    oracle().oracle_extender_seed(_ptr(q), len(q), _ptr(t), len(t), _ptr(m), xdrop, int(no_entropy), threshold, qs, ts, _ptr(out))
+    oracle().oracle_extender_seed(ptr(q), len(q), ptr(t), len(t), ptr(m), xdrop, int(no_entropy), threshold, qs, ts, ptr(out))
     return dict(zip(("query", "target", "length", "score", "kept", "total"), (int(v) for v in out)))
 
 
 def oracle_sort_unique(ssps):
     a = np.ascontiguousarray(ssps, dtype=SSP_DTYPE)
     out = np.zeros(len(a), dtype=SSP_DTYPE)
-    n = oracle().oracle_extender_sort_unique(_ptr(a), len(a), _ptr(out))
+    n = oracle().oracle_extender_sort_unique(ptr(a), len(a), ptr(out))
     return out[:n]
 
 
@@ -78,7 +62,7 @@ def oracle_run(query, target, matrix, xdrop, no_entropy, threshold, seeds):
     q, t, m = np.ascontiguousarray(query, np.int8), np.ascontiguousarray(target, np.int8), np.ascontiguousarray(matrix, np.int32)
     s = np.ascontiguousarray(seeds, dtype=SEED_DTYPE)
     out = np.zeros(max(len(s), 1), dtype=SSP_DTYPE)
-    n = oracle().oracle_extender_run(_ptr(q), len(q), _ptr(t), len(t), _ptr(m), xdrop, int(no_entropy), threshold, _ptr(s), len(s), _ptr(out))
+    n = oracle().oracle_extender_run(ptr(q), len(q), ptr(t), len(t), ptr(m), xdrop, int(no_entropy), threshold, ptr(s), len(s), ptr(out))
     return out[:n]
 
 
@@ -89,16 +73,14 @@ def ref_available():
 def ref_run(query, target, matrix, xdrop, no_entropy, threshold, seeds, reps=1, warmup=0):
     """The reference extender's device-pointer extend_async on cuda:0 -> (SSP array, ms of the `reps` calls that follow
     `warmup` untimed ones)."""
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_LIB)
-        _ref.ref_extender_run.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
-                                          C.c_int32, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_float), C.c_int32, C.c_int32]
+    L = load("_ref/libgwref_extender.so", {
+        "ref_extender_run": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                       C.c_int32, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_float), C.c_int32, C.c_int32])})
     q, t, m = np.ascontiguousarray(query, np.int8), np.ascontiguousarray(target, np.int8), np.ascontiguousarray(matrix, np.int32)
     s = np.ascontiguousarray(seeds, dtype=SEED_DTYPE)
     out = np.zeros(max(len(s), 1), dtype=SSP_DTYPE)
     n, ms = C.c_int32(0), C.c_float(0)
-    rc = _ref.ref_extender_run(_ptr(q), len(q), _ptr(t), len(t), _ptr(m), xdrop, int(no_entropy), threshold, _ptr(s), len(s), _ptr(out),
+    rc = L.ref_extender_run(ptr(q), len(q), ptr(t), len(t), ptr(m), xdrop, int(no_entropy), threshold, ptr(s), len(s), ptr(out),
                                C.byref(n), C.byref(ms), reps, warmup)
     if rc != 0:
         raise RuntimeError("reference extender failed")
@@ -158,5 +140,4 @@ def ssp_rows(a):
 
 
 def recorded_outputs():
-    with gzip.open(REF_OUTPUTS, "rt") as f:
-        return json.load(f)
+    return checker_lib.read_fixture(REF_OUTPUTS)

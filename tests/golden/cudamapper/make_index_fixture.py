@@ -4,13 +4,12 @@ IndexDescriptor hashes. Run once on a GPU with oracle/_ref/libgwref_index.so bui
 
     python tests/golden/cudamapper/make_index_fixture.py [output path]
 """
-import gzip
-import json
 import os
 import sys
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", ".."))
 import index_libs as il  # noqa: E402
+from checker_lib import write_fixture  # noqa: E402
 
 DESCRIPTORS = [(0, 0), (0, 1), (5, 10), (0xFFFFFFFF, 1), (123456, 0xFFFFFFFF), (7, 3000)]
 
@@ -24,9 +23,7 @@ def main():
         print(name, out["cases"][name]["sizes"], flush=True)
     for first, n in DESCRIPTORS:
         out["descriptor_hashes"].append([first, n, int(il.ref().ref_index_descriptor_hash(first, n))])
-    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
-    with gzip.open(path, "wt") as f:
-        json.dump(out, f, sort_keys=True)
+    write_fixture(path, out)
 
 
 if __name__ == "__main__":

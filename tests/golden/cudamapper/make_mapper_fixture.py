@@ -8,15 +8,13 @@ outputs. Needs an H100 and oracle/_ref/cudamapper (built by build() where the re
 (nothing fuses, so the reference's CIGARs, computed before fusion, sit on the right lines) and with at least two overlaps (with
 fewer overlaps than engines the reference's alignment batch size is 0 and it never returns). Every run has a timeout.
 """
-import gzip
-import json
 import os
 import sys
 import tempfile
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", ".."))
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", ".."))
 import mapper_libs as mp  # noqa: E402
+from checker_lib import write_fixture  # noqa: E402
 
 
 def main():
@@ -44,9 +42,7 @@ def main():
                 res[base + "_a2"] = mp.to_json(text)
                 print(name, base + "_a2", len(mp.sorted_lines(text)), flush=True)
             out["cases"][name] = res
-    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
-    with gzip.open(path, "wt") as f:
-        json.dump(out, f, sort_keys=True)
+    write_fixture(path, out)
 
 
 if __name__ == "__main__":

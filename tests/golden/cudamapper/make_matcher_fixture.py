@@ -7,13 +7,12 @@ GPU with oracle/_ref/libgwref_matcher.so built:
 Before it runs the reference on a case it asks the CPU oracle, and it refuses a case where both indices have unique
 representations but no anchor: the reference launches a zero-block grid there and aborts (DESIGN.md section 11.3).
 """
-import gzip
-import json
 import os
 import sys
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", ".."))
 import matcher_libs as ml  # noqa: E402
+from checker_lib import write_fixture  # noqa: E402
 
 
 def main():
@@ -27,9 +26,7 @@ def main():
         anchors, _, _ = ml.ref_run(c["reads"], qf, qn, tf, tn, c["k"], c["w"], c["hash"], c["F"])
         out["cases"][name] = ml.to_json(anchors, c["small"])
         print(name, len(anchors), flush=True)
-    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
-    with gzip.open(path, "wt") as f:
-        json.dump(out, f, sort_keys=True)
+    write_fixture(path, out)
 
 
 if __name__ == "__main__":

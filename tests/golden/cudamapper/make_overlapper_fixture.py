@@ -5,14 +5,12 @@ GPU with oracle/_ref/libgwref_overlapper.so built:
 
     python tests/golden/cudamapper/make_overlapper_fixture.py [output path]
 """
-import gzip
-import json
 import os
 import sys
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", ".."))
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", ".."))
 import overlapper_libs as ol  # noqa: E402
+from checker_lib import write_fixture  # noqa: E402
 
 
 def main():
@@ -24,9 +22,7 @@ def main():
     for name, lst in ol.post_lists().items():
         src = ol.from_rows(lst)
         out["post"][name] = {"drop%d" % d: ol.rows(ol.ref_post_process(src, bool(d))) for d in (0, 1)}
-    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
-    with gzip.open(path, "wt") as f:
-        json.dump(out, f, sort_keys=True)
+    write_fixture(path, out)
 
 
 if __name__ == "__main__":

@@ -5,14 +5,12 @@ code, so no GPU is needed; oracle/_ref/libgwref_rescue.so must be built:
 
     python tests/golden/cudamapper/make_rescue_fixture.py [output path]
 """
-import gzip
-import json
 import os
 import sys
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", ".."))
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", ".."))
 import rescue_libs as rl  # noqa: E402
+from checker_lib import write_fixture  # noqa: E402
 
 
 def main():
@@ -22,9 +20,7 @@ def main():
         out["cases"][name] = {p: rl.to_json(rl.ref_run(c["overlaps"], c["query_reads"], c["target_reads"], e, thr, c["mode"])[0], c["small"])
                               for p, (e, thr) in c["params"].items()}
         print(name, len(c["overlaps"]), flush=True)
-    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
-    with gzip.open(path, "wt") as f:
-        json.dump(out, f, sort_keys=True)
+    write_fixture(path, out)
 
 
 if __name__ == "__main__":

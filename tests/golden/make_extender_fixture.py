@@ -4,18 +4,14 @@ tests/extender_libs.synthetic_cases(). Needs a CUDA device. Run from the reposit
 
     python tests/golden/make_extender_fixture.py [output path]
 """
-import gzip
-import json
 import os
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
+import numpy as np
 
-import numpy as np  # noqa: E402
-
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import extender_libs as xl  # noqa: E402
+from checker_lib import write_fixture  # noqa: E402
 
 
 def main():
@@ -29,9 +25,7 @@ def main():
         res, _ = xl.ref_run(c["query"], c["target"], c["matrix"], c["xdrop"], c["no_entropy"], c["threshold"], c["seeds"])
         table[c["name"]] = xl.ssp_rows(res)
         print(c["name"], len(c["seeds"]), "seeds ->", len(res), "segments")
-    os.makedirs(os.path.dirname(out_path), exist_ok=True)
-    with gzip.GzipFile(out_path, "wb", mtime=0) as f:
-        f.write(json.dumps(table, sort_keys=True).encode())
+    write_fixture(out_path, table)
     print("wrote", out_path)
 
 

@@ -3,18 +3,16 @@ rebuilt for sm_90a) on deterministic synthetic windows, for every band mode. Run
     python tests/golden/make_reference_fixture.py
 The CPU test tests/test_oracle_poa.py::test_oracle_matches_reference_kernel_fixture re-creates the inputs from the recorded generator
 parameters and checks the CPU oracle against these outputs, which pins the oracle to the reference itself (not only to its KATs)."""
-import gzip
-import json
 import os
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np
-import oracle_lib as ol
-import ref_lib
-from genomeworks_b200 import synth
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import oracle_lib as ol  # noqa: E402
+import ref_lib  # noqa: E402
+from checker_lib import GOLDEN, write_fixture  # noqa: E402
+from genomeworks_b200 import synth  # noqa: E402
 
 GEN = dict(n_windows=12, backbone=600, reads=10, mut=12, ins=6, dele=6, seed0=4242)
 CASES = [dict(band_mode=0, band_width=256, max_pred=0), dict(band_mode=1, band_width=128, max_pred=0), dict(band_mode=2, band_width=128, max_pred=0),
@@ -31,7 +29,6 @@ for c in CASES:
     out["cases"].append(dict(c, status=[int(x) for x in ref["status"]], consensus=list(ref["consensus"]),
                              coverage=[[int(v) for v in cv] for cv in ref["coverage"]], oracle_with_ieee_division_identical=bool(same)))
     print(c, "reference ok windows:", int((np.array(ref["status"]) == 0).sum()), "oracle(ieee) identical:", same)
-path = os.path.join(ROOT, "tests", "golden", "reference_kernel_outputs.json.gz")
-with gzip.open(path, "wt") as f:
-    json.dump(out, f)
+path = os.path.join(GOLDEN, "reference_kernel_outputs.json.gz")
+write_fixture(path, out)
 print("wrote", path)

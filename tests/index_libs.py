@@ -7,23 +7,20 @@
 A result is a dict with the six arrays (numpy), "number_of_reads" and "longest" (number_of_basepairs_in_longest_read).
 """
 import ctypes as C
-import gzip
 import hashlib
 import os
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ORACLE_PATH = os.path.join(ROOT, "oracle", "liboracle_index.so")
-REF_PATH = os.path.join(ROOT, "oracle", "_ref", "libgwref_index.so")
-GOLDEN = os.path.join(ROOT, "tests", "golden", "cudamapper")
+import checker_lib
+from checker_lib import ROOT, load, ptr  # noqa: F401
+from genomeworks_b200.cudamapper import read_fasta
+
+GOLDEN = os.path.join(checker_lib.GOLDEN, "cudamapper")
 FIXTURE = os.path.join(GOLDEN, "reference_index_outputs.json.gz")
 ARRAYS = ("representations", "read_ids", "positions_in_reads", "directions_of_reads", "unique_representations",
           "first_occurrence_of_representations")
 DTYPES = (np.uint64, np.uint32, np.uint32, np.uint32, np.uint64, np.uint32)
-
-_oracle = None
-_ref = None
 
 
 def flatten(reads):
@@ -36,43 +33,32 @@ def flatten(reads):
 
 
 def oracle():
-    global _oracle
-    if _oracle is None:
-        L = C.CDLL(ORACLE_PATH)
-        L.oracle_index_run.restype = C.c_void_p
-        L.oracle_index_run.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_uint32, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_int32]
-        L.oracle_index_sizes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.oracle_index_get.argtypes = [C.c_void_p] * 7
-        L.oracle_index_free.argtypes = [C.c_void_p]
-        L.oracle_index_hash.restype = C.c_uint64
-        L.oracle_index_hash.argtypes = [C.c_uint64]
-        _oracle = L
-    return _oracle
+    return load("liboracle_index.so", {
+        "oracle_index_run": (C.c_void_p, [C.c_void_p, C.c_void_p, C.c_int64, C.c_uint32, C.c_int32, C.c_int32, C.c_int32, C.c_double,
+                                          C.c_int32]),
+        "oracle_index_sizes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+        "oracle_index_get": (C.c_int, [C.c_void_p] * 7),
+        "oracle_index_free": (C.c_int, [C.c_void_p]),
+        "oracle_index_hash": (C.c_uint64, [C.c_uint64])})
 
 
 def ref():
-    global _ref
-    if _ref is None:
-        L = C.CDLL(REF_PATH)
-        L.ref_index_run.restype = C.c_void_p
-        L.ref_index_run.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_uint32, C.c_uint32, C.c_int32, C.c_int32, C.c_int32, C.c_double,
-                                    C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
-        L.ref_index_sizes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.ref_index_get.argtypes = [C.c_void_p] * 7
-        L.ref_index_free.argtypes = [C.c_void_p]
-        L.ref_index_descriptor_hash.restype = C.c_uint64
-        L.ref_index_descriptor_hash.argtypes = [C.c_uint32, C.c_uint32]
-        _ref = L
-    return _ref
+    return load("_ref/libgwref_index.so", {
+        "ref_index_run": (C.c_void_p, [C.c_void_p, C.c_void_p, C.c_int64, C.c_uint32, C.c_uint32, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_double, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+        "ref_index_sizes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+        "ref_index_get": (C.c_int, [C.c_void_p] * 7),
+        "ref_index_free": (C.c_int, [C.c_void_p]),
+        "ref_index_descriptor_hash": (C.c_uint64, [C.c_uint32, C.c_uint32])})
 
 
 def _collect(L, prefix, h, nscalars):
     sizes = np.zeros(3, dtype=np.int64)
     scalars = np.zeros(nscalars, dtype=np.uint32)
-    getattr(L, prefix + "_sizes")(h, sizes.ctypes.data_as(C.c_void_p), scalars.ctypes.data_as(C.c_void_p))
+    getattr(L, prefix + "_sizes")(h, ptr(sizes), ptr(scalars))
     ne, nu, nf = (int(x) for x in sizes)
     out = {name: np.zeros(n, dtype=dt) for name, n, dt in zip(ARRAYS, (ne, ne, ne, ne, nu, nf), DTYPES)}
-    getattr(L, prefix + "_get")(h, *[out[a].ctypes.data_as(C.c_void_p) for a in ARRAYS])
+    getattr(L, prefix + "_get")(h, *[ptr(out[a]) for a in ARRAYS])
     getattr(L, prefix + "_free")(h)
     return out, scalars
 
@@ -80,7 +66,7 @@ def _collect(L, prefix, h, nscalars):
 def oracle_run(reads, first_read_id, k, w, hash_representations=True, filtering_parameter=1.0, literal=False):
     """The oracle on the reads of the index (read i has id first_read_id + i)."""
     bases, offsets = flatten(reads)
-    h = oracle().oracle_index_run(bases.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), len(reads), first_read_id, k, w,
+    h = oracle().oracle_index_run(ptr(bases), ptr(offsets), len(reads), first_read_id, k, w,
                                   1 if hash_representations else 0, filtering_parameter, 1 if literal else 0)
     if not h:
         raise ValueError("invalid k or w")
@@ -94,7 +80,7 @@ def ref_run(all_reads, first_read, number_of_reads, k, w, hash_representations=T
     (result, device_ms, e2e_ms) for the reps timed calls."""
     bases, offsets = flatten(all_reads)
     dms, ems = C.c_float(), C.c_float()
-    h = ref().ref_index_run(bases.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), len(all_reads), first_read, number_of_reads,
+    h = ref().ref_index_run(ptr(bases), ptr(offsets), len(all_reads), first_read, number_of_reads,
                             k, w, 1 if hash_representations else 0, filtering_parameter, reps, warmup, C.byref(dms), C.byref(ems))
     if not h:
         raise RuntimeError("reference index failed")
@@ -145,23 +131,6 @@ SMALL_FILES = {  # the (k, w) pairs the reference's own index tests use on each 
 }
 
 
-def read_fasta(path):
-    opener = gzip.open if path.endswith(".gz") else open
-    seqs, cur = [], None
-    with opener(path, "rb") as f:
-        for line in f:
-            line = line.rstrip(b"\r\n")
-            if line.startswith(b">"):
-                if cur is not None:
-                    seqs.append(b"".join(cur))
-                cur = []
-            elif cur is not None:
-                cur.append(line)
-    if cur is not None:
-        seqs.append(b"".join(cur))
-    return seqs
-
-
 def random_reads(seed, n, lo, hi, alphabet=b"ACGT"):
     rng = np.random.default_rng(seed)
     al = np.frombuffer(alphabet, dtype=np.uint8)
@@ -209,9 +178,7 @@ def cases():
 
 
 def load_fixture():
-    import json
-    with gzip.open(FIXTURE, "rt") as f:
-        return json.load(f)
+    return checker_lib.read_fixture(FIXTURE)
 
 
 def to_json(result, small):

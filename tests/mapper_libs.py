@@ -1,7 +1,7 @@
 """Inputs, option sets and runners shared by the cudamapper tool's tests, its fixture generator and tools/bench_mapper.py.
 
 - build/cudamapper: this engine's tool (built by build());
-- oracle/_ref/cudamapper: the unmodified reference tool, built by build() where the reference sources exist (oracle/mapper.mk);
+- oracle/_ref/cudamapper: the unmodified reference tool, built by build() where the reference sources exist (oracle/Makefile);
   only the fixture generator and the benchmark run it;
 - oracle/_ref/libgwref_mapper_utils.so: the reference's print_paf, group_reads_into_indices and parser order (host code), used
   by the CPU tests where it exists.
@@ -13,7 +13,6 @@ one genome with every other read reverse-complemented.
 import ctypes as C
 import gzip
 import hashlib
-import json
 import os
 import subprocess
 import sys
@@ -21,12 +20,13 @@ import sys
 import numpy as np
 
 import index_libs as il
+from checker_lib import REF_DIR, load, ptr, read_fixture
 
 ROOT = il.ROOT
 GOLDEN = il.GOLDEN
 TOOL = os.path.join(ROOT, "build", "cudamapper")
-REF_TOOL = os.path.join(ROOT, "oracle", "_ref", "cudamapper")
-REF_UTILS = os.path.join(ROOT, "oracle", "_ref", "libgwref_mapper_utils.so")
+REF_TOOL = os.path.join(REF_DIR, "cudamapper")
+REF_UTILS = os.path.join(REF_DIR, "libgwref_mapper_utils.so")
 FIXTURE = os.path.join(GOLDEN, "reference_mapper_outputs.json.gz")
 SMALL = 3000  # outputs of at most this many lines are stored line by line, larger ones as a count and a SHA-256
 MEMORY = ["-m", "4"]  # an explicit pool of 4 GiB: the GPU machines are shared
@@ -121,8 +121,7 @@ def matches(text, stored):
 
 
 def load_fixture():
-    with gzip.open(FIXTURE, "rt") as f:
-        return json.load(f)
+    return read_fixture(FIXTURE)
 
 
 def cigar_lengths(cigar):
@@ -144,21 +143,11 @@ def cigar_lengths(cigar):
     return q, t
 
 
-_utils = None
-
-
 def ref_utils():
-    global _utils
-    if _utils is None:
-        L = C.CDLL(REF_UTILS)
-        L.ref_print_paf.argtypes = [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]
-        L.ref_print_paf.restype = C.c_int64
-        L.ref_group_reads_into_indices.argtypes = [C.c_char_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64]
-        L.ref_group_reads_into_indices.restype = C.c_int64
-        L.ref_parser_names.argtypes = [C.c_char_p, C.c_uint32, C.c_void_p, C.c_int64]
-        L.ref_parser_names.restype = C.c_int64
-        _utils = L
-    return _utils
+    return load("_ref/libgwref_mapper_utils.so", {
+        "ref_print_paf": (C.c_int64, [C.c_char_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64]),
+        "ref_group_reads_into_indices": (C.c_int64, [C.c_char_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64]),
+        "ref_parser_names": (C.c_int64, [C.c_char_p, C.c_uint32, C.c_void_p, C.c_int64])})
 
 
 def ref_print_paf(query_path, target_path, overlaps, cigars, kmer_size):
@@ -168,7 +157,7 @@ def ref_print_paf(query_path, target_path, overlaps, cigars, kmer_size):
     if cigars is not None:
         bufs = [C.create_string_buffer(c.encode()) for c in cigars]
         cg = (C.c_char_p * max(1, len(bufs)))(*[C.cast(b, C.c_char_p) for b in bufs])
-    args = (query_path.encode(), target_path.encode(), ov.ctypes.data_as(C.c_void_p), len(ov), C.cast(cg, C.c_void_p) if cg is not None else None,
+    args = (query_path.encode(), target_path.encode(), ptr(ov), len(ov), C.cast(cg, C.c_void_p) if cg is not None else None,
             kmer_size)
     n = L.ref_print_paf(*args, None, 0)
     out = C.create_string_buffer(max(1, n))
@@ -181,7 +170,7 @@ def ref_group_reads_into_indices(path, max_basepairs):
     cap = 1 << 16
     first = np.zeros(cap, dtype=np.uint32)
     count = np.zeros(cap, dtype=np.uint32)
-    k = L.ref_group_reads_into_indices(path.encode(), max_basepairs, first.ctypes.data_as(C.c_void_p), count.ctypes.data_as(C.c_void_p), cap)
+    k = L.ref_group_reads_into_indices(path.encode(), max_basepairs, ptr(first), ptr(count), cap)
     return [(int(first[i]), int(count[i])) for i in range(k)]
 
 

@@ -8,55 +8,33 @@ Anchors are (n, 4) uint32 arrays: query read id, target read id, query position,
 index_libs (the index oracle), whose reads, renumbering and fixtures this module reuses.
 """
 import ctypes as C
-import gzip
 import hashlib
-import json
 import os
 
 import numpy as np
 
 import index_libs as il
+from checker_lib import load, ptr, read_fixture
 
 ROOT = il.ROOT
-ORACLE_PATH = os.path.join(ROOT, "oracle", "liboracle_matcher.so")
-REF_PATH = os.path.join(ROOT, "oracle", "_ref", "libgwref_matcher.so")
 FIXTURE = os.path.join(il.GOLDEN, "reference_matcher_outputs.json.gz")
 INT_MAX = 2**31 - 1
 
-_oracle = None
-_ref = None
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
-
 
 def oracle():
-    global _oracle
-    if _oracle is None:
-        L = C.CDLL(ORACLE_PATH)
-        L.oracle_matcher_count.restype = C.c_int64
-        L.oracle_matcher_count.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
-        L.oracle_matcher_run.restype = C.c_int64
-        L.oracle_matcher_run.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
-                                         C.c_void_p, C.c_void_p, C.c_int64]
-        _oracle = L
-    return _oracle
+    return load("liboracle_matcher.so", {
+        "oracle_matcher_count": (C.c_int64, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+        "oracle_matcher_run": (C.c_int64, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64])})
 
 
 def ref():
-    global _ref
-    if _ref is None:
-        L = C.CDLL(REF_PATH)
-        L.ref_matcher_run.restype = C.c_void_p
-        L.ref_matcher_run.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32, C.c_int32,
-                                      C.c_int32, C.c_double, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
-        L.ref_matcher_size.restype = C.c_int64
-        L.ref_matcher_size.argtypes = [C.c_void_p]
-        L.ref_matcher_get.argtypes = [C.c_void_p, C.c_void_p]
-        L.ref_matcher_free.argtypes = [C.c_void_p]
-        _ref = L
-    return _ref
+    return load("_ref/libgwref_matcher.so", {
+        "ref_matcher_run": (C.c_void_p, [C.c_void_p, C.c_void_p, C.c_int64, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32,
+                                         C.c_int32, C.c_int32, C.c_double, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+        "ref_matcher_size": (C.c_int64, [C.c_void_p]),
+        "ref_matcher_get": (C.c_int, [C.c_void_p, C.c_void_p]),
+        "ref_matcher_free": (C.c_int, [C.c_void_p])})
 
 
 def _index_arrays(s):
@@ -68,7 +46,7 @@ def oracle_count(q, t):
     """Anchors of two sketches (dicts with the index arrays, as index_libs.oracle_run returns them), counted without building."""
     qu, qf, _, _ = _index_arrays(q)
     tu, tf, _, _ = _index_arrays(t)
-    return int(oracle().oracle_matcher_count(_p(qu), len(qu), _p(qf), _p(tu), len(tu), _p(tf)))
+    return int(oracle().oracle_matcher_count(ptr(qu), len(qu), ptr(qf), ptr(tu), len(tu), ptr(tf)))
 
 
 def oracle_run(q, t):
@@ -77,7 +55,7 @@ def oracle_run(q, t):
     tu, tf, tr, tp = _index_arrays(t)
     n = oracle_count(q, t)
     out = np.zeros((n, 4), dtype=np.uint32)
-    got = oracle().oracle_matcher_run(_p(qu), len(qu), _p(qf), _p(qr), _p(qp), _p(tu), len(tu), _p(tf), _p(tr), _p(tp), _p(out), n)
+    got = oracle().oracle_matcher_run(ptr(qu), len(qu), ptr(qf), ptr(qr), ptr(qp), ptr(tu), len(tu), ptr(tf), ptr(tr), ptr(tp), ptr(out), n)
     assert got == n
     return out
 
@@ -88,12 +66,12 @@ def ref_run(all_reads, q_first, q_n, t_first, t_n, k, w, hash_representations=Tr
     non-empty indices that share no representation (the reference aborts there)."""
     bases, offsets = il.flatten(all_reads)
     dms, ems = C.c_float(), C.c_float()
-    h = ref().ref_matcher_run(_p(bases), _p(offsets), len(all_reads), q_first, q_n, t_first, t_n, k, w, 1 if hash_representations else 0,
+    h = ref().ref_matcher_run(ptr(bases), ptr(offsets), len(all_reads), q_first, q_n, t_first, t_n, k, w, 1 if hash_representations else 0,
                               filtering_parameter, reps, warmup, C.byref(dms), C.byref(ems))
     if not h:
         raise RuntimeError("reference matcher failed")
     out = np.zeros((ref().ref_matcher_size(h), 4), dtype=np.uint32)
-    ref().ref_matcher_get(h, _p(out))
+    ref().ref_matcher_get(h, ptr(out))
     ref().ref_matcher_free(h)
     return out, dms.value, ems.value
 
@@ -164,8 +142,7 @@ def sketches(c):
 
 
 def load_fixture():
-    with gzip.open(FIXTURE, "rt") as f:
-        return json.load(f)
+    return read_fixture(FIXTURE)
 
 
 def to_json(anchors, small):

@@ -1,32 +1,15 @@
 """ctypes bindings for the CPU oracle (oracle/liboracle.so). TEST INFRASTRUCTURE ONLY."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_ORACLE_DIR = os.path.join(ROOT, "oracle")
-_lib = None
+from checker_lib import load, ptr
 
 FDIV_T = C.CFUNCTYPE(C.c_float, C.c_float, C.c_float)
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        path = os.path.join(_ORACLE_DIR, "liboracle.so")
-        srcs = [os.path.join(_ORACLE_DIR, f) for f in ("poa_oracle.cpp", "myers_oracle.cpp", "global_oracle.cpp")]
-        if (not os.path.exists(path)) or any(os.path.getmtime(s) > os.path.getmtime(path) for s in srcs):
-            subprocess.check_call(["make", "-C", _ORACLE_DIR, "oracle"], stdout=subprocess.DEVNULL)
-        _lib = C.CDLL(path)
-        _lib.oracle_graph_create.restype = C.c_void_p
-        _lib.oracle_set_fdiv.argtypes = [C.c_void_p]
-    return _lib
-
-
-def _p(a, t):
-    return a.ctypes.data_as(C.POINTER(t)) if a is not None else None
+    return load("liboracle.so", {"oracle_graph_create": (C.c_void_p, None), "oracle_set_fdiv": (C.c_int, [C.c_void_p])})
 
 
 def batch_config(max_seq=1024, max_seq_per_poa=100, band_width=256, band_mode=0, adaptive_storage_factor=2.0,
@@ -34,7 +17,7 @@ def batch_config(max_seq=1024, max_seq_per_poa=100, band_width=256, band_mode=0,
     out = np.zeros(8, dtype=np.int32)
     lib().oracle_poa_batch_config(C.c_int32(max_seq), C.c_int32(max_seq_per_poa), C.c_int32(band_width), C.c_int32(band_mode),
                                   C.c_float(adaptive_storage_factor), C.c_float(graph_length_factor), C.c_int32(max_pred_dist),
-                                  _p(out, C.c_int32))
+                                  ptr(out))
     return out
 
 
@@ -63,10 +46,10 @@ def poa_run(windows, cfg8, msa=False, gap=-8, mismatch=-6, match=8, weights=None
     if weights is not None:
         w = np.ascontiguousarray(np.concatenate([np.asarray(x, dtype=np.int8) for win in weights for x in win] + [np.zeros(1, np.int8)]))
     cfg8 = np.ascontiguousarray(cfg8, dtype=np.int32)
-    lib().oracle_poa_run(C.c_int32(n), _p(win_nseq, C.c_int32), _p(seq_len, C.c_int32), _p(data, C.c_char), _p(w, C.c_int8),
-                         _p(cfg8, C.c_int32), C.c_int32(1 if msa else 0), C.c_int32(gap), C.c_int32(mismatch), C.c_int32(match),
-                         _p(cons, C.c_char), _p(cov, C.c_uint16), _p(status, C.c_int32), _p(msa_buf, C.c_char) if msa else None,
-                         _p(cells, C.c_int64), _p(nodes, C.c_int32))
+    lib().oracle_poa_run(C.c_int32(n), ptr(win_nseq), ptr(seq_len), ptr(data), ptr(w),
+                         ptr(cfg8), C.c_int32(1 if msa else 0), C.c_int32(gap), C.c_int32(mismatch), C.c_int32(match),
+                         ptr(cons), ptr(cov), ptr(status), ptr(msa_buf) if msa else None,
+                         ptr(cells), ptr(nodes))
     out_c, out_cov = [], []
     for i in range(n):
         s = bytes(cons[i]).split(b"\0", 1)[0].decode()
@@ -90,8 +73,8 @@ def poa_row_stats(windows, cfg8, gap=-8, mismatch=-6, match=8):
     win_nseq, seq_len, data = flatten_windows(windows)
     out = np.zeros((len(windows), 4), dtype=np.int64)
     cfg8 = np.ascontiguousarray(cfg8, dtype=np.int32)
-    lib().oracle_poa_row_stats(C.c_int32(len(windows)), _p(win_nseq, C.c_int32), _p(seq_len, C.c_int32), _p(data, C.c_char),
-                               _p(cfg8, C.c_int32), C.c_int32(gap), C.c_int32(mismatch), C.c_int32(match), _p(out, C.c_int64))
+    lib().oracle_poa_row_stats(C.c_int32(len(windows)), ptr(win_nseq), ptr(seq_len), ptr(data),
+                               ptr(cfg8), C.c_int32(gap), C.c_int32(mismatch), C.c_int32(match), ptr(out))
     return out
 
 
@@ -112,13 +95,13 @@ class OGraph:
         sg = np.array(sorted_graph, dtype=np.int32) if sorted_graph is not None else None
         iw = np.ascontiguousarray(in_w_raw, dtype=np.uint16) if in_w_raw is not None else None
         cv = np.array(coverage, dtype=np.uint16) if coverage is not None else None
-        self.h = C.c_void_p(lib().oracle_graph_create(C.c_int32(n), C.c_int32(max_nodes), _p(nodes_a, C.c_uint8), _p(sg, C.c_int32),
-                                                      _p(off, C.c_int32), _p(adj_a, C.c_int32), _p(iw, C.c_uint16), _p(cv, C.c_uint16)))
+        self.h = C.c_void_p(lib().oracle_graph_create(C.c_int32(n), C.c_int32(max_nodes), ptr(nodes_a), ptr(sg),
+                                                      ptr(off), ptr(adj_a), ptr(iw), ptr(cv)))
         if alignments is not None:
             for i, a in enumerate(alignments):
                 if len(a):
                     aa = np.array(a, dtype=np.int32)
-                    lib().oracle_graph_set_alignments(self.h, C.c_int32(i), C.c_int32(len(a)), _p(aa, C.c_int32))
+                    lib().oracle_graph_set_alignments(self.h, C.c_int32(i), C.c_int32(len(a)), ptr(aa))
 
     def __del__(self):
         try:
@@ -133,7 +116,7 @@ class OGraph:
         res = []
         buf = np.zeros(64, dtype=np.int32)
         for i in range(self.node_count()):
-            k = lib().oracle_graph_out_edges(self.h, C.c_int32(i), _p(buf, C.c_int32))
+            k = lib().oracle_graph_out_edges(self.h, C.c_int32(i), ptr(buf))
             res.append([int(x) for x in buf[:k]])
         return res
 
@@ -142,17 +125,17 @@ class OGraph:
         ar = np.array(alignment_read, dtype=np.int32)
         rd = np.frombuffer(read.encode() if isinstance(read, str) else bytes(read), dtype=np.uint8).copy()
         bw = np.array(base_weights, dtype=np.int8)
-        return lib().oracle_graph_add_alignment(self.h, C.c_int32(len(ag)), _p(ag, C.c_int32), _p(ar, C.c_int32), _p(rd, C.c_uint8),
-                                                _p(bw, C.c_int8))
+        return lib().oracle_graph_add_alignment(self.h, C.c_int32(len(ag)), ptr(ag), ptr(ar), ptr(rd),
+                                                ptr(bw))
 
     def nw(self, read, mode, band_width=128, max_nodes=3072, matrix_seq_dim=136, gap=-8, mismatch=-6, match=8):
         rd = np.frombuffer((read.encode() if isinstance(read, str) else bytes(read)) + b"\0\0\0\0\0\0\0\0", dtype=np.uint8).copy()
         L = len(rd) - 8
         ag = np.zeros(max_nodes * 2 + L + 16, dtype=np.int32)
         ar = np.zeros_like(ag)
-        r = lib().oracle_graph_nw(self.h, _p(rd, C.c_uint8), C.c_int32(L), C.c_int32(mode), C.c_int32(band_width), C.c_int32(max_nodes),
-                                  C.c_int32(matrix_seq_dim), C.c_int32(gap), C.c_int32(mismatch), C.c_int32(match), _p(ag, C.c_int32),
-                                  _p(ar, C.c_int32))
+        r = lib().oracle_graph_nw(self.h, ptr(rd), C.c_int32(L), C.c_int32(mode), C.c_int32(band_width), C.c_int32(max_nodes),
+                                  C.c_int32(matrix_seq_dim), C.c_int32(gap), C.c_int32(mismatch), C.c_int32(match), ptr(ag),
+                                  ptr(ar))
         if r < 0:
             return r, None, None
         return r, [int(x) for x in ag[:r]], [int(x) for x in ar[:r]]
@@ -160,7 +143,7 @@ class OGraph:
     def consensus(self, max_consensus=2048):
         buf = np.zeros(max_consensus + 2, dtype=np.uint8)
         cov = np.zeros(max_consensus + 2, dtype=np.uint16)
-        st = lib().oracle_graph_consensus(self.h, C.c_int32(max_consensus), _p(buf, C.c_char), _p(cov, C.c_uint16))
+        st = lib().oracle_graph_consensus(self.h, C.c_int32(max_consensus), ptr(buf), ptr(cov))
         s = bytes(buf).split(b"\0", 1)[0].decode()
         return st, s, cov[:len(s)].copy()
 
@@ -174,7 +157,7 @@ def topsort(out_edges):
         off[i + 1] = len(adj)
     adj_a = np.array(adj + [0], dtype=np.int32)
     out = np.zeros(n, dtype=np.int32)
-    lib().oracle_topsort(C.c_int32(n), _p(off, C.c_int32), _p(adj_a, C.c_int32), _p(out, C.c_int32))
+    lib().oracle_topsort(C.c_int32(n), ptr(off), ptr(adj_a), ptr(out))
     return [int(x) for x in out]
 
 
@@ -219,8 +202,8 @@ def myers_align(query, target, max_bandwidth, max_elements_per_matrix=0):
     opt = C.c_int32(0)
     cells = C.c_int64(0)
     k = lib().oracle_myers_banded_align(C.c_char_p(q), C.c_int32(len(q)), C.c_char_p(t), C.c_int32(len(t)), C.c_int32(max_bandwidth),
-                                        C.c_int64(max_elements_per_matrix), C.byref(status), C.byref(opt), _p(actions, C.c_int8),
-                                        _p(runs, C.c_int32), C.byref(cells))
+                                        C.c_int64(max_elements_per_matrix), C.byref(status), C.byref(opt), ptr(actions),
+                                        ptr(runs), C.byref(cells))
     a, r = actions[:k].copy(), runs[:k].copy()
     return dict(status=status.value, is_optimal=opt.value, actions=a, runs=r, cigar=cigar_from_runs(a, r),
                 cigar_extended=cigar_from_runs(a, r, True), edit_distance=edit_distance_from_runs(a, r), cells=cells.value)
@@ -250,8 +233,7 @@ def hirschberg_myers_align(query, target, max_query_length=None):
     mq = len(q) if max_query_length is None else max_query_length
     out = np.zeros(len(q) + len(t) + 1, dtype=np.int8)
     failed = C.c_int32(0)
-    lib().oracle_hirschberg_myers_align.restype = C.c_int32
-    n = lib().oracle_hirschberg_myers_align(q, C.c_int32(len(q)), t, C.c_int32(len(t)), C.c_int32(mq), _p(out, C.c_int8), C.byref(failed))
+    n = lib().oracle_hirschberg_myers_align(q, C.c_int32(len(q)), t, C.c_int32(len(t)), C.c_int32(mq), ptr(out), C.byref(failed))
     return out[:n].copy(), bool(failed.value)
 
 
@@ -260,8 +242,7 @@ def myers_full_align(query, target):
     q = query.encode() if isinstance(query, str) else bytes(query)
     t = target.encode() if isinstance(target, str) else bytes(target)
     out = np.zeros(len(q) + len(t) + 1, dtype=np.int8)
-    lib().oracle_myers_full_align.restype = C.c_int32
-    n = lib().oracle_myers_full_align(q, C.c_int32(len(q)), t, C.c_int32(len(t)), _p(out, C.c_int8))
+    n = lib().oracle_myers_full_align(q, C.c_int32(len(q)), t, C.c_int32(len(t)), ptr(out))
     return out[:n].copy()
 
 
@@ -277,8 +258,7 @@ def global_stats(algorithm, query, target, max_query_length=None):
     mq = len(q) if max_query_length is None else max_query_length
     alg = {"hirschberg_myers": 0, "myers": 1, "ukkonen": 2}[algorithm]
     out = np.zeros(len(GLOBAL_STATS), dtype=np.int64)
-    lib().oracle_global_stats.restype = C.c_int32
-    failed = lib().oracle_global_stats(C.c_int32(alg), q, C.c_int32(len(q)), t, C.c_int32(len(t)), C.c_int32(mq), _p(out, C.c_int64))
+    failed = lib().oracle_global_stats(C.c_int32(alg), q, C.c_int32(len(q)), t, C.c_int32(len(t)), C.c_int32(mq), ptr(out))
     res = {k: int(v) for k, v in zip(GLOBAL_STATS, out)}
     res["failed"] = bool(failed)
     return res
@@ -289,6 +269,5 @@ def ukkonen_align(query, target, p=100):
     q = query.encode() if isinstance(query, str) else bytes(query)
     t = target.encode() if isinstance(target, str) else bytes(target)
     out = np.zeros(len(q) + len(t) + 1, dtype=np.int8)
-    lib().oracle_ukkonen_align.restype = C.c_int32
-    n = lib().oracle_ukkonen_align(q, C.c_int32(len(q)), t, C.c_int32(len(t)), C.c_int32(p), _p(out, C.c_int8))
+    n = lib().oracle_ukkonen_align(q, C.c_int32(len(q)), t, C.c_int32(len(t)), C.c_int32(p), ptr(out))
     return out[:n].copy()

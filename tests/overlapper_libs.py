@@ -9,18 +9,15 @@ cudamapper.OVERLAP_DTYPE arrays. The cases are anchor sequences given to both si
 plays no part.
 """
 import ctypes as C
-import gzip
 import hashlib
-import json
 import os
 
 import numpy as np
 
 import index_libs as il
+from checker_lib import load, ptr, read_fixture
 
 ROOT = il.ROOT
-ORACLE_PATH = os.path.join(ROOT, "oracle", "liboracle_overlapper.so")
-REF_PATH = os.path.join(ROOT, "oracle", "_ref", "libgwref_overlapper.so")
 FIXTURE = os.path.join(il.GOLDEN, "reference_overlapper_outputs.json.gz")
 INT_MAX = 2**31 - 1
 FIELDS = ("query_read_id", "target_read_id", "query_start_position_in_read", "target_start_position_in_read", "query_end_position_in_read",
@@ -41,45 +38,25 @@ PARAMS = {
     "negative_length": (True, 3, -250, 1000, 0.0),        # size_t(-250): no overlap is that long
 }
 
-_oracle = None
-_ref = None
-
-
 def dtype():
     from genomeworks_b200.cudamapper import OVERLAP_DTYPE
     return OVERLAP_DTYPE
 
 
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
 def oracle():
-    global _oracle
-    if _oracle is None:
-        L = C.CDLL(ORACLE_PATH)
-        L.oracle_overlapper_run.restype = C.c_int64
-        L.oracle_overlapper_run.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_float, C.c_void_p, C.c_void_p,
-                                            C.c_int64]
-        _oracle = L
-    return _oracle
+    return load("liboracle_overlapper.so", {
+        "oracle_overlapper_run": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_float, C.c_void_p,
+                                              C.c_void_p, C.c_int64])})
 
 
 def ref():
-    global _ref
-    if _ref is None:
-        L = C.CDLL(REF_PATH)
-        L.ref_overlapper_run.restype = C.c_void_p
-        L.ref_overlapper_run.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_float, C.c_int32, C.c_int32,
-                                         C.c_void_p, C.c_void_p]
-        L.ref_overlapper_size.restype = C.c_int64
-        L.ref_overlapper_size.argtypes = [C.c_void_p]
-        L.ref_overlapper_get.argtypes = [C.c_void_p, C.c_void_p]
-        L.ref_overlapper_free.argtypes = [C.c_void_p]
-        L.ref_post_process.restype = C.c_int64
-        L.ref_post_process.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64]
-        _ref = L
-    return _ref
+    return load("_ref/libgwref_overlapper.so", {
+        "ref_overlapper_run": (C.c_void_p, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_float, C.c_int32,
+                                            C.c_int32, C.c_void_p, C.c_void_p]),
+        "ref_overlapper_size": (C.c_int64, [C.c_void_p]),
+        "ref_overlapper_get": (C.c_int, [C.c_void_p, C.c_void_p]),
+        "ref_overlapper_free": (C.c_int, [C.c_void_p]),
+        "ref_post_process": (C.c_int64, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64])})
 
 
 def anchors_array(rows):
@@ -96,7 +73,7 @@ def oracle_run(anchors, params, div=None):
     a = anchors_array(anchors)
     cap = max(len(a) // 3, 1)
     out = np.zeros(cap, dtype=dtype())
-    n = oracle().oracle_overlapper_run(_p(a), len(a), int(a2a), mr, mol, mbpr, frac, C.cast(div, C.c_void_p) if div else None, _p(out), cap)
+    n = oracle().oracle_overlapper_run(ptr(a), len(a), int(a2a), mr, mol, mbpr, frac, C.cast(div, C.c_void_p) if div else None, ptr(out), cap)
     assert n <= cap
     return out[:n].copy()
 
@@ -106,11 +83,11 @@ def ref_run(anchors, params, reps=1, warmup=0):
     a2a, mr, mol, mbpr, frac = params
     a = anchors_array(anchors)
     dms, ems = C.c_float(), C.c_float()
-    h = ref().ref_overlapper_run(_p(a), len(a), int(a2a), mr, mol, mbpr, frac, reps, warmup, C.byref(dms), C.byref(ems))
+    h = ref().ref_overlapper_run(ptr(a), len(a), int(a2a), mr, mol, mbpr, frac, reps, warmup, C.byref(dms), C.byref(ems))
     if not h:
         raise RuntimeError("reference overlapper failed")
     out = np.zeros(ref().ref_overlapper_size(h), dtype=dtype())
-    ref().ref_overlapper_get(h, _p(out))
+    ref().ref_overlapper_get(h, ptr(out))
     ref().ref_overlapper_free(h)
     return out, dms.value, ems.value
 
@@ -118,7 +95,7 @@ def ref_run(anchors, params, reps=1, warmup=0):
 def ref_post_process(overlaps, drop):
     src = np.ascontiguousarray(overlaps, dtype=dtype())
     out = np.zeros(len(src) + len(src) // 2, dtype=dtype())
-    n = ref().ref_post_process(_p(src), len(src), int(drop), _p(out), len(out))
+    n = ref().ref_post_process(ptr(src), len(src), int(drop), ptr(out), len(out))
     assert n <= len(out)
     return out[:n].copy()
 
@@ -163,8 +140,7 @@ def matches(overlaps, stored):
 
 
 def load_fixture():
-    with gzip.open(FIXTURE, "rt") as f:
-        return json.load(f)
+    return read_fixture(FIXTURE)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------

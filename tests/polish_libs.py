@@ -7,21 +7,17 @@ the seeded inputs the polisher's tests share.
   CudaPoaBatch.add_poa_group per group, oracle_stitch.
 """
 import ctypes as C
-import os
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ORACLE_PATH = os.path.join(ROOT, "oracle", "liboracle_polish.so")
+from checker_lib import ROOT, load, ptr  # noqa: F401
+
 KEYS = ("draft_window_first", "candidates", "used", "group_draft", "group_window", "win_nseq", "seq_len", "seq_data")
 OVERLAP_DTYPE = np.dtype({"names": ["query_read_id", "target_read_id", "query_start_position_in_read", "target_start_position_in_read",
                                     "query_end_position_in_read", "target_end_position_in_read", "relative_strand", "num_residues",
                                     "overlap_complete"],
                           "formats": ["<u4", "<u4", "<u4", "<u4", "<u4", "<u4", "u1", "<u4", "u1"],
                           "offsets": [0, 4, 8, 12, 16, 20, 24, 28, 32], "itemsize": 36})
-
-_oracle = None
-
 
 class _View(C.Structure):
     _fields_ = [("n_drafts", C.c_int64), ("n_windows", C.c_int64), ("draft_window_first", C.c_void_p), ("candidates", C.c_void_p),
@@ -31,18 +27,13 @@ class _View(C.Structure):
 
 
 def oracle():
-    global _oracle
-    if _oracle is None:
-        L = C.CDLL(ORACLE_PATH)
-        L.oracle_polish_groups.restype = C.c_int
-        L.oracle_polish_groups.argtypes = [C.c_void_p, C.c_int64, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_char_p,
-                                           C.c_void_p, C.c_int64, C.c_int32, C.c_int32]
-        L.oracle_polish_view.argtypes = [C.POINTER(_View)]
-        L.oracle_polish_stitch.argtypes = [C.c_char_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_char_p, C.c_void_p]
-        L.oracle_polish_stitched.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
-                                             C.POINTER(C.c_int64)]
-        _oracle = L
-    return _oracle
+    return load("liboracle_polish.so", {
+        "oracle_polish_groups": (C.c_int, [C.c_void_p, C.c_int64, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_char_p,
+                                           C.c_void_p, C.c_int64, C.c_int32, C.c_int32]),
+        "oracle_polish_view": (C.c_int, [C.POINTER(_View)]),
+        "oracle_polish_stitch": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_char_p, C.c_void_p]),
+        "oracle_polish_stitched": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                             C.POINTER(C.c_int64)])})
 
 
 def _array(ptr, n, dtype):
@@ -74,8 +65,8 @@ def oracle_groups(overlaps, cigars, drafts, reads, window_length, max_depth):
     text, toffs = cigar_text(cigars)
     db, doffs = _flat(drafts)
     rb, roffs = _flat(reads)
-    rc = oracle().oracle_polish_groups(ov.ctypes.data_as(C.c_void_p), len(ov), text, toffs.ctypes.data_as(C.c_void_p), db,
-                                       doffs.ctypes.data_as(C.c_void_p), len(doffs) - 1, rb, roffs.ctypes.data_as(C.c_void_p), len(roffs) - 1,
+    rc = oracle().oracle_polish_groups(ptr(ov), len(ov), text, ptr(toffs), db,
+                                       ptr(doffs), len(doffs) - 1, rb, ptr(roffs), len(roffs) - 1,
                                        window_length, max_depth)
     if rc != 0:
         return rc, None
@@ -100,8 +91,8 @@ def oracle_stitch(drafts, window_length, used, group_status, consensus):
     used = np.ascontiguousarray(used, dtype=np.int32)
     st = np.ascontiguousarray(group_status, dtype=np.int32)
     ctext, coffs = _flat(consensus)
-    oracle().oracle_polish_stitch(db, doffs.ctypes.data_as(C.c_void_p), len(doffs) - 1, window_length, used.ctypes.data_as(C.c_void_p),
-                                  st.ctypes.data_as(C.c_void_p), ctext, coffs.ctypes.data_as(C.c_void_p))
+    oracle().oracle_polish_stitch(db, ptr(doffs), len(doffs) - 1, window_length, ptr(used),
+                                  ptr(st), ctext, ptr(coffs))
     text, offs, outcome, status, n = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int64()
     oracle().oracle_polish_stitched(C.byref(text), C.byref(offs), C.byref(outcome), C.byref(status), C.byref(n))
     o = _array(offs.value, len(doffs), np.int64)

@@ -7,28 +7,19 @@ from proven parts (DESIGN.md section 15.5).
   with its weights, the oracle's stitching.
 """
 import ctypes as C
-import os
 
 import numpy as np
 
 import polish_libs as pl
-
-ORACLE_Q_PATH = os.path.join(pl.ROOT, "oracle", "liboracle_polish_q.so")
-
-_oracle = None
+from checker_lib import load, ptr
 
 
 def oracle():
-    global _oracle
-    if _oracle is None:
-        L = C.CDLL(ORACLE_Q_PATH)
-        L.oracle_polish_groups_q.restype = C.c_int
-        L.oracle_polish_groups_q.argtypes = [C.c_void_p, C.c_int64, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_char_p,
-                                             C.c_void_p, C.c_int64, C.c_char_p, C.c_double, C.c_int32, C.c_int32]
-        L.oracle_polish_view.argtypes = [C.POINTER(pl._View)]
-        L.oracle_polish_weights.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
-        _oracle = L
-    return _oracle
+    return load("liboracle_polish_q.so", {
+        "oracle_polish_groups_q": (C.c_int, [C.c_void_p, C.c_int64, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_char_p,
+                                             C.c_void_p, C.c_int64, C.c_char_p, C.c_double, C.c_int32, C.c_int32]),
+        "oracle_polish_view": (C.c_int, [C.POINTER(pl._View)]),
+        "oracle_polish_weights": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)])})
 
 
 def oracle_groups_q(overlaps, cigars, drafts, reads, qualities, threshold, window_length, max_depth):
@@ -40,8 +31,8 @@ def oracle_groups_q(overlaps, cigars, drafts, reads, qualities, threshold, windo
     qb, qoffs = pl._flat(qualities)
     assert np.array_equal(roffs, qoffs), "one quality string per read, as long as the read"
     L = oracle()
-    rc = L.oracle_polish_groups_q(ov.ctypes.data_as(C.c_void_p), len(ov), text, toffs.ctypes.data_as(C.c_void_p), db,
-                                  doffs.ctypes.data_as(C.c_void_p), len(doffs) - 1, rb, roffs.ctypes.data_as(C.c_void_p), len(roffs) - 1, qb,
+    rc = L.oracle_polish_groups_q(ptr(ov), len(ov), text, ptr(toffs), db,
+                                  ptr(doffs), len(doffs) - 1, rb, ptr(roffs), len(roffs) - 1, qb,
                                   threshold, window_length, max_depth)
     if rc != 0:
         return rc, None

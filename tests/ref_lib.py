@@ -2,18 +2,15 @@
 unmodified reference sources), and the stored outputs of those libraries the tests compare against. TEST / BASELINE
 INFRASTRUCTURE ONLY."""
 import ctypes as C
-import gzip
 import hashlib
 import json
 import os
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_DIR = os.path.join(ROOT, "oracle", "_ref")
-GOLDEN_OUTPUTS = os.path.join(ROOT, "tests", "golden", "reference_outputs.json.gz")
-_gwref = None
-_spoa = None
+from checker_lib import GOLDEN, REF_DIR, ROOT, load, ptr, read_fixture, write_fixture  # noqa: F401
+
+GOLDEN_OUTPUTS = os.path.join(GOLDEN, "reference_outputs.json.gz")
 _golden = None
 
 
@@ -36,13 +33,12 @@ def recorded(key, run):
     out = os.environ.get("GWB200_RECORD_REFERENCE")
     if out:
         value = json.loads(json.dumps(run()))
-        table = json.load(gzip.open(out, "rt")) if os.path.exists(out) else {}
+        table = read_fixture(out) if os.path.exists(out) else {}
         table[key] = value
-        with gzip.open(out, "wt") as f:
-            json.dump(table, f, sort_keys=True)
+        write_fixture(out, table)
         return value
     if _golden is None:
-        _golden = json.load(gzip.open(GOLDEN_OUTPUTS, "rt"))
+        _golden = read_fixture(GOLDEN_OUTPUTS)
     return _golden[key]
 
 
@@ -55,22 +51,11 @@ def have_spoa():
 
 
 def gwref():
-    global _gwref
-    if _gwref is None:
-        _gwref = C.CDLL(os.path.join(REF_DIR, "libgwref.so"))
-    return _gwref
+    return load("_ref/libgwref.so", {})
 
 
 def spoa():
-    global _spoa
-    if _spoa is None:
-        _spoa = C.CDLL(os.path.join(REF_DIR, "libspoa_ref.so"))
-        _spoa.spoa_consensus_run.restype = C.c_double
-    return _spoa
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p) if a is not None else None
+    return load("_ref/libspoa_ref.so", {"spoa_consensus_run": (C.c_double, None)})
 
 
 def ref_poa_run(win_nseq, seq_len, seq_data, max_seq_size, max_seq_per_poa, band_width, band_mode, adaptive_storage_factor=2.0,
@@ -91,11 +76,11 @@ def ref_poa_run(win_nseq, seq_len, seq_data, max_seq_size, max_seq_per_poa, band
     err = C.create_string_buffer(1024)
     if weights is not None:
         weights = np.ascontiguousarray(weights, dtype=np.int8)
-    rc = gwref().ref_poa_run(C.c_int32(n), _p(win_nseq), _p(seq_len), _p(seq_data), _p(weights), C.c_int32(max_seq_size), C.c_int32(max_seq_per_poa),
+    rc = gwref().ref_poa_run(C.c_int32(n), ptr(win_nseq), ptr(seq_len), ptr(seq_data), ptr(weights), C.c_int32(max_seq_size), C.c_int32(max_seq_per_poa),
                              C.c_int32(band_width), C.c_int32(band_mode), C.c_float(adaptive_storage_factor), C.c_float(graph_length_factor),
                              C.c_int32(max_pred_dist), C.c_int32(2 if msa else 1), C.c_int32(gap), C.c_int32(mismatch), C.c_int32(match),
-                             C.c_double(mem_fraction), C.c_int32(max_windows_per_batch), _p(cons), _p(cov), _p(status), _p(msa_buf),
-                             C.byref(mc_out), _p(timings), err, C.c_int32(1024))
+                             C.c_double(mem_fraction), C.c_int32(max_windows_per_batch), ptr(cons), ptr(cov), ptr(status), ptr(msa_buf),
+                             C.byref(mc_out), ptr(timings), err, C.c_int32(1024))
     if rc != 0:
         raise RuntimeError("reference cudapoa failed: " + err.value.decode())
     assert mc_out.value == mc
@@ -131,9 +116,9 @@ def ref_aligner_run(q_len, q_data, t_len, t_data, max_bandwidth, max_device_memo
     ce = np.zeros((n, cigar_stride), dtype=np.uint8)
     timings = np.zeros(2, dtype=np.float64)
     err = C.create_string_buffer(1024)
-    rc = gwref().ref_aligner_run(C.c_int32(n), _p(q_len), _p(q_data), _p(t_len), _p(t_data), C.c_int32(max_bandwidth),
-                                 C.c_int64(max_device_memory), _p(status), _p(opt), _p(ed), _p(cb), _p(ce), C.c_int32(cigar_stride),
-                                 _p(timings), err, C.c_int32(1024))
+    rc = gwref().ref_aligner_run(C.c_int32(n), ptr(q_len), ptr(q_data), ptr(t_len), ptr(t_data), C.c_int32(max_bandwidth),
+                                 C.c_int64(max_device_memory), ptr(status), ptr(opt), ptr(ed), ptr(cb), ptr(ce), C.c_int32(cigar_stride),
+                                 ptr(timings), err, C.c_int32(1024))
     if rc != 0:
         raise RuntimeError("reference cudaaligner failed: " + err.value.decode())
     return dict(status=status, is_optimal=opt, edit_distance=ed,
@@ -148,8 +133,8 @@ def spoa_consensus(win_nseq, seq_len, seq_data, n_threads=0, match=8, mismatch=-
     n = len(win_nseq)
     buf = np.zeros((n, stride), dtype=np.uint8) if want_strings else None
     cells = C.c_double(0)
-    secs = spoa().spoa_consensus_run(C.c_int32(n), _p(win_nseq), _p(seq_len), _p(seq_data), C.c_int32(match), C.c_int32(mismatch),
-                                     C.c_int32(gap), C.c_int32(n_threads), _p(buf), C.c_int32(stride), C.byref(cells))
+    secs = spoa().spoa_consensus_run(C.c_int32(n), ptr(win_nseq), ptr(seq_len), ptr(seq_data), C.c_int32(match), C.c_int32(mismatch),
+                                     C.c_int32(gap), C.c_int32(n_threads), ptr(buf), C.c_int32(stride), C.byref(cells))
     cons = [bytes(buf[i]).split(b"\0", 1)[0].decode() for i in range(n)] if want_strings else None
     return dict(seconds=secs, cells=cells.value, consensus=cons, threads=n_threads or spoa().spoa_hardware_threads())
 
@@ -170,9 +155,9 @@ def ref_global_aligner_run(q_len, q_data, t_len, t_data, algorithm, max_query_le
     ce = np.zeros((n, cigar_stride), dtype=np.uint8)
     timings = np.zeros(2, dtype=np.float64)
     err = C.create_string_buffer(1024)
-    rc = gwref().ref_global_aligner_run(C.c_int32(n), _p(q_len), _p(q_data), _p(t_len), _p(t_data), C.c_int32(algorithm),
-                                        C.c_int32(max_query_length), C.c_int32(max_target_length), _p(status), _p(opt), _p(ed), _p(cb), _p(ce),
-                                        C.c_int32(cigar_stride), _p(timings), err, C.c_int32(1024))
+    rc = gwref().ref_global_aligner_run(C.c_int32(n), ptr(q_len), ptr(q_data), ptr(t_len), ptr(t_data), C.c_int32(algorithm),
+                                        C.c_int32(max_query_length), C.c_int32(max_target_length), ptr(status), ptr(opt), ptr(ed), ptr(cb), ptr(ce),
+                                        C.c_int32(cigar_stride), ptr(timings), err, C.c_int32(1024))
     if rc != 0:
         raise RuntimeError("reference global aligner failed: " + err.value.decode())
     return dict(status=status, is_optimal=opt, edit_distance=ed,
@@ -185,7 +170,7 @@ def spoa_msa(seqs, match=8, mismatch=-6, gap=-8, stride=8192):
     lens = np.array([len(x) for x in seqs], dtype=np.int32)
     data = np.frombuffer(("".join(seqs) + "\0").encode(), dtype=np.uint8)
     out = np.zeros((len(seqs), stride), dtype=np.uint8)
-    w = spoa().spoa_msa_run(C.c_int32(len(seqs)), _p(lens), _p(data), C.c_int32(match), C.c_int32(mismatch), C.c_int32(gap), _p(out),
+    w = spoa().spoa_msa_run(C.c_int32(len(seqs)), ptr(lens), ptr(data), C.c_int32(match), C.c_int32(mismatch), C.c_int32(gap), ptr(out),
                             C.c_int32(stride))
     if w < 0:
         raise RuntimeError("stride too small")

@@ -8,18 +8,15 @@ A case is a query read list, a target read list (the same list object for all-vs
 1: extend once) and named (extension, required_similarity) parameter sets.
 """
 import ctypes as C
-import gzip
-import json
 import os
 
 import numpy as np
 
 import index_libs as il
 import overlapper_libs as ol
+from checker_lib import load, ptr, read_fixture
 
 ROOT = il.ROOT
-ORACLE_PATH = os.path.join(ROOT, "oracle", "liboracle_rescue.so")
-REF_PATH = os.path.join(ROOT, "oracle", "_ref", "libgwref_rescue.so")
 FIXTURE = os.path.join(il.GOLDEN, "reference_rescue_outputs.json.gz")
 UNIT_FASTA = os.path.join(il.GOLDEN, "overlap_extension_unit.fasta")
 RESCUE, EXTEND_ONCE = 0, 1
@@ -41,38 +38,16 @@ PARAMS = {
     "thr_third": (50, THIRD),
 }
 
-_oracle = None
-_ref = None
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
-def _lib(path, name):
-    L = C.CDLL(path)
-    f = getattr(L, name)
-    f.restype = C.c_int
-    f.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_int32]
-    return L
+# overlaps, their count, query bases, offsets and count, target bases, offsets and count, extension, threshold, mode
+_RUN_ARGS = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_int32]
 
 
 def oracle():
-    global _oracle
-    if _oracle is None:
-        _oracle = _lib(ORACLE_PATH, "oracle_rescue_run")
-    return _oracle
+    return load("liboracle_rescue.so", {"oracle_rescue_run": (C.c_int, _RUN_ARGS)})
 
 
 def ref():
-    global _ref
-    if _ref is None:
-        L = C.CDLL(REF_PATH)
-        L.ref_rescue_run.restype = C.c_int
-        L.ref_rescue_run.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
-                                     C.c_float, C.c_int32, C.c_void_p]
-        _ref = L
-    return _ref
+    return load("_ref/libgwref_rescue.so", {"ref_rescue_run": (C.c_int, _RUN_ARGS + [C.c_void_p])})
 
 
 def flat(reads):
@@ -91,7 +66,7 @@ def _args(overlaps, query_reads, target_reads):
 def oracle_run(overlaps, query_reads, target_reads, extension, threshold, mode=RESCUE):
     """(0, updated overlaps) or (-1, the overlaps unchanged) for the arguments the contract rejects."""
     out, (qb, qo, nq, tb, to, nt) = _args(overlaps, query_reads, target_reads)
-    rc = oracle().oracle_rescue_run(_p(out), len(out), _p(qb), _p(qo), nq, _p(tb), _p(to), nt, extension, threshold, mode)
+    rc = oracle().oracle_rescue_run(ptr(out), len(out), ptr(qb), ptr(qo), nq, ptr(tb), ptr(to), nt, extension, threshold, mode)
     return rc, out
 
 
@@ -99,15 +74,14 @@ def ref_run(overlaps, query_reads, target_reads, extension, threshold, mode=RESC
     """(updated overlaps, the reference's host wall ms)."""
     out, (qb, qo, nq, tb, to, nt) = _args(overlaps, query_reads, target_reads)
     ms = C.c_float()
-    rc = ref().ref_rescue_run(_p(out), len(out), _p(qb), _p(qo), nq, _p(tb), _p(to), nt, extension, threshold, mode, C.byref(ms))
+    rc = ref().ref_rescue_run(ptr(out), len(out), ptr(qb), ptr(qo), nq, ptr(tb), ptr(to), nt, extension, threshold, mode, C.byref(ms))
     if rc != 0:
         raise RuntimeError("the reference rescue threw")
     return out, ms.value
 
 
 def load_fixture():
-    with gzip.open(FIXTURE, "rt") as f:
-        return json.load(f)
+    return read_fixture(FIXTURE)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
