@@ -267,6 +267,8 @@ def lib():
     L.gwb200_gapped_extender_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float)]
     L.gwb200_gapped_extender_last_live_cells.argtypes = [C.c_void_p]
     L.gwb200_gapped_extender_last_live_cells.restype = C.c_int64
+    L.gwb200_gapped_extender_set_skip_covered.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    L.gwb200_gapped_extender_last_skip_stats.argtypes = [C.c_void_p, C.c_void_p]
     L.gwb200_seeder_create_with_allocator.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                                       C.c_void_p]
     L.gwb200_seeder_destroy.argtypes = [C.c_void_p]
@@ -292,6 +294,8 @@ def lib():
     L.gwb200_genome_aligner_cigar_bytes.restype = C.c_int64
     L.gwb200_genome_aligner_get_cigars.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
     L.gwb200_genome_aligner_last_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_genome_aligner_set_skip_covered.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    L.gwb200_genome_aligner_last_skip_stats.argtypes = [C.c_void_p, C.c_void_p]
     L.gwb200_index_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int64, C.c_uint32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_double, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     L.gwb200_index_wait.argtypes = [C.c_void_p]

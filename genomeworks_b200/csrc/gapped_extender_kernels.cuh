@@ -380,5 +380,72 @@ __global__ void ssp_anchors_kernel(const SspIn* __restrict__ ssps, int32_t n, in
     }
 }
 
+// Skip-covered mode (DESIGN.md section 18): the anchors still to process form one device list of anchor indices in processing
+// order. A round gathers its first anchors, runs pass 1 on them, and the host resolves it; the M runs of the alignments it kept
+// then remove every later anchor they cover from the list.
+
+// Processing order of scored segment pairs: score descending as an ascending unsigned key; the SSP index as the value, so a
+// stable radix sort puts ties in index order.
+__global__ void ssp_order_keys_kernel(const SspIn* __restrict__ ssps, int32_t n, uint32_t* __restrict__ keys, int32_t* __restrict__ idx)
+{
+    for (int32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x)
+    {
+        keys[k] = ~(static_cast<uint32_t>(ssps[k].score) ^ 0x80000000u);
+        idx[k]  = k;
+    }
+}
+
+// Processing order of host anchors: the order given.
+__global__ void iota_kernel(int32_t n, int32_t* __restrict__ idx)
+{
+    for (int32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x)
+        idx[k] = k;
+}
+
+// The round's anchors: out[k] = anchors[list[k]], k < r. Pass 1 runs over their sides 2k (left) and 2k + 1 (right).
+__global__ void round_anchors_kernel(const AnchorD* __restrict__ anchors, const int32_t* __restrict__ list, int32_t r, AnchorD* __restrict__ out)
+{
+    for (int32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < r; k += gridDim.x * blockDim.x)
+        out[k] = anchors[list[k]];
+}
+
+// One M run of kept paths: query q aligned with target q + diag for q in [begin, end). Runs are sorted by (diag, begin), and
+// the runs of one diagonal are disjoint.
+struct MRun
+{
+    long long diag;
+    int32_t begin;
+    int32_t end;
+};
+
+// keep[k] = 1 when anchor list[k] lies on no run; one thread per anchor, a binary search for the last run at or before it.
+__global__ void covered_kernel(const AnchorD* __restrict__ anchors, const int32_t* __restrict__ list, int32_t n, const MRun* __restrict__ runs,
+                               int32_t nruns, uint8_t* __restrict__ keep)
+{
+    for (int32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x)
+    {
+        const AnchorD a    = anchors[list[k]];
+        const long long d  = static_cast<long long>(a.target) - a.query;
+        const long long q  = a.query;
+        int32_t lo = 0, hi = nruns; // the first run after (d, q)
+        while (lo < hi)
+        {
+            const int32_t mid = (lo + hi) >> 1;
+            const MRun m      = runs[mid];
+            if (m.diag < d || (m.diag == d && m.begin <= q))
+                lo = mid + 1;
+            else
+                hi = mid;
+        }
+        bool covered = false;
+        if (lo > 0)
+        {
+            const MRun m = runs[lo - 1];
+            covered      = m.diag == d && q < m.end;
+        }
+        keep[k] = covered ? 0 : 1;
+    }
+}
+
 } // namespace gapped
 } // namespace gwb200

@@ -6,7 +6,8 @@
 // appends the segments it keeps for every block to one buffer (grown between blocks), and one sort and unique over all of
 // them gives exactly the result of one extender call over all the seeds. The unique segments go to the gapped extender on the
 // device; their alignments come back with CIGARs, and the host maps minus-strand query intervals to forward coordinates and
-// counts the PAF columns.
+// counts the PAF columns. In skip-covered mode (DESIGN.md section 18) the gapped extender of each pair and strand runs the
+// sequential rule in its own coordinates.
 
 #include "../../include/gwb200.h"
 #include "common.cuh"
@@ -90,6 +91,7 @@ struct gwb200_genome_aligner
     std::vector<int64_t> offsets{0};
     float stage_ms[kStages] = {};
     int64_t n_seeds = 0, n_ssps = 0;
+    int64_t skip_stats[5] = {}; // the gapped extender's, summed over pairs and strands
 
     ~gwb200_genome_aligner()
     {
@@ -218,6 +220,11 @@ int align_pair(gwb200_genome_aligner* a, int32_t ti, int32_t qi, int32_t strand,
     gwb200_gapped_extender_last_ms(a->gapped, &ms1, &ms2);
     a->stage_ms[kGapped1] += std::max(0.f, ms1);
     a->stage_ms[kGapped2] += std::max(0.f, ms2);
+    int64_t stats[5];
+    if ((rc = gwb200_gapped_extender_last_skip_stats(a->gapped, stats)) < 0)
+        return rc;
+    for (int k = 0; k < 5; ++k)
+        a->skip_stats[k] += stats[k];
     const int32_t n = gwb200_gapped_extender_num_results(a->gapped);
     if (n < 0)
         return n;
@@ -295,6 +302,7 @@ void clear(gwb200_genome_aligner* a)
     a->offsets.assign(1, 0);
     std::fill(a->stage_ms, a->stage_ms + kStages, 0.f);
     a->n_seeds = a->n_ssps = 0;
+    std::fill(a->skip_stats, a->skip_stats + 5, int64_t(0));
 }
 
 int run(gwb200_genome_aligner* a, const int8_t* targets, const int64_t* toff, int32_t nt, const int8_t* queries, const int64_t* qoff, int32_t nq)
@@ -482,6 +490,25 @@ int gwb200_genome_aligner_last_stats(const gwb200_genome_aligner* a, float* stag
     counts[0] = a->n_seeds;
     counts[1] = a->n_ssps;
     counts[2] = static_cast<int64_t>(a->results.size());
+    return 0;
+}
+
+int gwb200_genome_aligner_set_skip_covered(gwb200_genome_aligner* a, int32_t on, int32_t round_anchors)
+{
+    if (round_anchors < 0)
+        return GWB200_EXT_INVALID_INPUT;
+    if (!a)
+        return set_error(GWB200_E_INVALID_ARGUMENT, "null genome aligner");
+    return gwb200_gapped_extender_set_skip_covered(a->gapped, on, round_anchors);
+}
+
+int gwb200_genome_aligner_last_skip_stats(const gwb200_genome_aligner* a, int64_t* out)
+{
+    if (!a || !out)
+        return set_error(GWB200_E_INVALID_ARGUMENT, "null argument");
+    if (!a->ready)
+        return set_error(GWB200_E_RUNTIME, "no finished run: call gwb200_genome_aligner_run first");
+    std::copy(a->skip_stats, a->skip_stats + 5, out);
     return 0;
 }
 

@@ -153,6 +153,18 @@ ANCHOR_DTYPE = SEED_DTYPE
 GAPPED_DTYPE = np.dtype([("score", np.int64), ("anchor", np.int32), ("has_cigar", np.int32), ("query_begin", np.uint32),
                          ("query_end", np.uint32), ("target_begin", np.uint32), ("target_end", np.uint32)])
 DEFAULT_GAPPED_BUDGET = 1 << 30
+SKIP_STATS = ("extended", "skipped", "speculative", "traced", "rounds")
+
+
+def _skip_args(skip_covered, round_anchors):
+    """Checks the skip-covered arguments (DESIGN.md section 18) before any device work; -> (on, round_anchors) as ints."""
+    if not isinstance(skip_covered, (bool, np.bool_)):
+        raise TypeError("skip_covered must be True or False")
+    if isinstance(round_anchors, (bool, np.bool_)) or not isinstance(round_anchors, (int, np.integer)):
+        raise TypeError("round_anchors must be an integer")
+    if not 0 <= int(round_anchors) < (1 << 31):
+        raise ValueError("round_anchors must lie in [0, 2^31 - 1]; 0 picks the device's default")
+    return int(bool(skip_covered)), int(round_anchors)
 
 
 class GappedXDrop:
@@ -160,9 +172,10 @@ class GappedXDrop:
     into one alignment with a CIGAR (M / I / D, I consuming the query)."""
 
     def __init__(self, score_matrix, gap_open, gap_extend, ydrop, budget_bytes=DEFAULT_GAPPED_BUDGET, stream=None, device_id=0,
-                 allocator=None):
+                 allocator=None, skip_covered=False, round_anchors=0):
         mat = np.ascontiguousarray(np.asarray(score_matrix, dtype=np.int64).ravel())
         self._h = C.c_void_p()
+        skip = _skip_args(skip_covered, round_anchors)
         for name, v, hi in (("gap_open", gap_open, 1 << 24), ("gap_extend", gap_extend, 1 << 24), ("ydrop", ydrop, 1 << 28)):
             if not 0 <= int(v) <= hi:
                 raise ValueError("%s must lie in [0, %d]" % (name, hi))
@@ -180,6 +193,16 @@ class GappedXDrop:
             raise ValueError("invalid gapped extender parameters")
         check(rc)
         self._keep = ()
+        if skip[0]:
+            self.set_skip_covered(*skip)
+
+    def set_skip_covered(self, on=True, round_anchors=0):
+        """Skip-covered mode for later calls (DESIGN.md section 18): an anchor on the path of an alignment kept earlier in the
+        same call is not extended. round_anchors (anchors per device round, 0 = the device's default) never changes an output.
+        Raises RuntimeError while a call is pending."""
+        on, round_anchors = _skip_args(bool(on), round_anchors)
+        if check(lib().gwb200_gapped_extender_set_skip_covered(self._h, C.c_int32(on), C.c_int32(round_anchors))) == invalid_operation:
+            raise RuntimeError("an extend call is pending: sync() it first")
 
     def extend_async(self, query, target, threshold, anchors):
         """Host-pointer extension of `anchors` (structured array with query / target fields); returns a StatusType
@@ -231,6 +254,12 @@ class GappedXDrop:
     def last_live_cells(self):
         return check(lib().gwb200_gapped_extender_last_live_cells(self._h))
 
+    def last_skip_stats(self):
+        """Of the last finished call: {extended, skipped, speculative, traced, rounds} (DESIGN.md section 18)."""
+        out = np.zeros(len(SKIP_STATS), dtype=np.int64)
+        check(lib().gwb200_gapped_extender_last_skip_stats(self._h, out.ctypes.data_as(C.c_void_p)))
+        return dict(zip(SKIP_STATS, (int(v) for v in out)))
+
     def close(self):
         if self._h:
             lib().gwb200_gapped_extender_destroy(self._h)
@@ -244,10 +273,11 @@ class GappedXDrop:
 
 
 def create_gapped_extender(score_matrix, gap_open, gap_extend, ydrop, budget_bytes=DEFAULT_GAPPED_BUDGET, stream=None, device_id=0,
-                           allocator=None):
+                           allocator=None, skip_covered=False, round_anchors=0):
     """A GappedXDrop over the 8 x 8 (or 64-entry) substitution matrix, row = target code, column = query code. Parameters
-    outside their ranges raise ValueError before any device work; without a CUDA device this raises RuntimeError."""
-    return GappedXDrop(score_matrix, gap_open, gap_extend, ydrop, budget_bytes, stream, device_id, allocator)
+    outside their ranges raise ValueError before any device work; without a CUDA device this raises RuntimeError.
+    skip_covered=True starts it in skip-covered mode (GappedXDrop.set_skip_covered)."""
+    return GappedXDrop(score_matrix, gap_open, gap_extend, ydrop, budget_bytes, stream, device_id, allocator, skip_covered, round_anchors)
 
 
 # Seeding (DESIGN.md section 17): the hits of LASTZ's 12-of-19 spaced seed, in the global order of include/gwb200.h.
@@ -365,10 +395,11 @@ def _records(seqs):
 class GenomeAligner:
     """The aligner with fixed parameters; run(targets, queries) aligns every query record against every target record."""
 
-    def __init__(self, strand="both", stream=None, device_id=0, allocator=None, **params):
+    def __init__(self, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, round_anchors=0, **params):
         from ._lib import GenomeAlignerParams
         if strand not in STRANDS:
             raise ValueError("strand must be one of %s" % ", ".join(STRANDS))
+        skip = _skip_args(skip_covered, round_anchors)
         p = default_genome_params()
         unknown = set(params) - set(p)
         if unknown:
@@ -391,6 +422,8 @@ class GenomeAligner:
         if rc == invalid_input:
             raise ValueError("invalid genome aligner parameters")
         check(rc)
+        if skip[0]:
+            check(lib().gwb200_genome_aligner_set_skip_covered(self._h, C.c_int32(skip[0]), C.c_int32(skip[1])))
 
     def run(self, targets, queries):
         """-> (GENOME_DTYPE records, CIGAR strings, '' where has_cigar is 0). Blocking."""
@@ -417,6 +450,13 @@ class GenomeAligner:
         check(lib().gwb200_genome_aligner_last_stats(self._h, ms.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p)))
         return dict(zip(STAGES, (float(v) for v in ms))), dict(zip(("seeds", "ssps", "alignments"), (int(v) for v in counts)))
 
+    def last_skip_stats(self):
+        """Of the last run, summed over every pair and strand: {extended, skipped, speculative, traced, rounds} of the gapped
+        stage (DESIGN.md section 18)."""
+        out = np.zeros(len(SKIP_STATS), dtype=np.int64)
+        check(lib().gwb200_genome_aligner_last_skip_stats(self._h, out.ctypes.data_as(C.c_void_p)))
+        return dict(zip(SKIP_STATS, (int(v) for v in out)))
+
     def close(self):
         if self._h:
             lib().gwb200_genome_aligner_destroy(self._h)
@@ -429,13 +469,14 @@ class GenomeAligner:
             pass
 
 
-def align_genomes(targets, queries, strand="both", stream=None, device_id=0, allocator=None, **params):
+def align_genomes(targets, queries, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, **params):
     """Aligns every query record against every target record on the plus strand, the minus strand or both. targets and queries
     are lists of sequences (str or int8 codes). Keyword parameters override gwb200_genome_aligner_default_params: score_matrix,
     xdrop, ssp_threshold, gap_open, gap_extend, ydrop, gapped_threshold, transition, block_size, traceback_budget. Returns
     (GENOME_DTYPE records, CIGAR strings); query coordinates are forward for both strands and minus-strand CIGARs read the
-    target forward. Bad parameters raise ValueError before any device work."""
-    al = GenomeAligner(strand, stream, device_id, allocator, **params)
+    target forward. Bad parameters raise ValueError before any device work. skip_covered=True does not extend the anchors that
+    lie on an alignment kept earlier for the same pair and strand (DESIGN.md section 18)."""
+    al = GenomeAligner(strand, stream, device_id, allocator, skip_covered, **params)
     try:
         return al.run(targets, queries)
     finally:

@@ -105,6 +105,18 @@ public:
         results_.clear();
     }
 
+    /// Skip-covered mode for later calls (DESIGN.md section 18): an anchor on the path of an alignment kept earlier in the same
+    /// call is not extended. round_anchors: anchors per device round (0: the device's default); it never changes an output.
+    /// Throws std::invalid_argument for round_anchors < 0 and std::logic_error while a call is pending.
+    void set_skip_covered(bool on, int32_t round_anchors = 0)
+    {
+        const int rc = detail::check(gwb200_gapped_extender_set_skip_covered(h_, on ? 1 : 0, round_anchors));
+        if (rc == GWB200_EXT_INVALID_INPUT)
+            throw std::invalid_argument("round_anchors must be >= 0");
+        if (rc == GWB200_EXT_INVALID_OPERATION)
+            throw std::logic_error("an extend call is pending");
+    }
+
 private:
     static void* pool_alloc(void* user, int64_t bytes)
     {
@@ -138,6 +150,17 @@ inline std::unique_ptr<GappedExtender> create_gapped_extender(const int32_t* h_s
 {
     return std::unique_ptr<GappedExtender>(
         new GappedExtender(h_score_mat, score_mat_dim, gap_open, gap_extend, ydrop, budget_bytes, stream, device_id, allocator));
+}
+
+/// The same, started in skip-covered mode when skip_covered is true (GappedExtender::set_skip_covered).
+inline std::unique_ptr<GappedExtender> create_gapped_extender(const int32_t* h_score_mat, int32_t score_mat_dim, int32_t gap_open, int32_t gap_extend,
+                                                              int32_t ydrop, int64_t budget_bytes, cudaStream_t stream, int32_t device_id,
+                                                              DefaultDeviceAllocator allocator, bool skip_covered)
+{
+    std::unique_ptr<GappedExtender> x = create_gapped_extender(h_score_mat, score_mat_dim, gap_open, gap_extend, ydrop, budget_bytes, stream,
+                                                               device_id, allocator);
+    x->set_skip_covered(skip_covered);
+    return x;
 }
 
 } // namespace cudaextender

@@ -456,6 +456,16 @@ int gwb200_gapped_extender_reset(gwb200_gapped_extender* extender);
  * and the live cells of every side of every anchor. */
 int gwb200_gapped_extender_last_ms(const gwb200_gapped_extender* extender, float* pass1_ms, float* pass2_ms);
 int64_t gwb200_gapped_extender_last_live_cells(const gwb200_gapped_extender* extender);
+/* Skip-covered mode (DESIGN.md section 18), off by default; it holds for later calls until turned off. Anchors are processed
+ * in the order given (host calls) or by SSP score descending, ties by SSP index (device calls). An anchor that lies on an M
+ * position of an alignment kept earlier in the same call is skipped; every other one is extended as above. Results come in
+ * the order they are kept, and the live cells count the extended anchors only. round_anchors: anchors per device round (0:
+ * half the resident warps of pass 1); it never changes an output. invalid_input for round_anchors < 0, invalid_operation while
+ * a call is pending. */
+int gwb200_gapped_extender_set_skip_covered(gwb200_gapped_extender* extender, int32_t on, int32_t round_anchors);
+/* Of the last finished call: out[5] = the anchors extended, the anchors skipped, the skipped anchors that ran through pass 1,
+ * the alignments traced by pass 2, and the rounds (default mode: n, 0, 0, the traced alignments, 1 when n > 0). */
+int gwb200_gapped_extender_last_skip_stats(const gwb200_gapped_extender* extender, int64_t* out);
 
 /* ------------------------------------------------------------------------------------------------
  * cudaextender, seeding stage (DESIGN.md section 17): the hits of LASTZ's 12-of-19 spaced seed 1110100110010101111 between a
@@ -557,6 +567,11 @@ int gwb200_genome_aligner_get_cigars(const gwb200_genome_aligner* aligner, char*
 /* Of the last run, summed over every pair and strand: device ms of index, count, write, ungapped, gapped pass 1 and gapped
  * pass 2 (stage_ms[6]), and the seeds, the unique segments and the alignments (counts[3]). */
 int gwb200_genome_aligner_last_stats(const gwb200_genome_aligner* aligner, float* stage_ms, int64_t* counts);
+/* Puts the aligner's gapped extender in skip-covered mode (gwb200_gapped_extender_set_skip_covered) for later runs. Coverage
+ * never crosses a (pair, strand), and minus-strand anchors are tested in the strand's own coordinates. */
+int gwb200_genome_aligner_set_skip_covered(gwb200_genome_aligner* aligner, int32_t on, int32_t round_anchors);
+/* gwb200_gapped_extender_last_skip_stats of the last run, summed over every pair and strand. */
+int gwb200_genome_aligner_last_skip_stats(const gwb200_genome_aligner* aligner, int64_t* out);
 
 /* ------------------------------------------------------------------------------------------------
  * cudamapper (minimizer index)

@@ -1,7 +1,8 @@
 """Genome aligner benchmark: one JSON line per workload, with the aligner's defaults (both strands, transitions, the sample
 matrix, LASTZ-style gapped parameters, blocks of 2^25 seeds).
 
-    python tools/bench_genome_aligner.py [--steps K] [--warmup W] [--workloads sample,assembly]
+    python tools/bench_genome_aligner.py [--steps K] [--warmup W] [--workloads sample,assembly] [--modes default,skip]
+                                         [--skip-covered]
 
 Workloads:
   sample    the golden sample (one 250 kb record) against itself;
@@ -13,6 +14,11 @@ Each line: the per-stage device ms of the last run (CUDA events summed over pair
 gapped pass 1 and pass 2), the seeds, unique segments and alignments, seeds/s of the seeding stage (count + write) and of the
 write pass alone with its bytes/s (8 bytes written per seed), and the wall time of a whole run (host clock, mean of `steps` runs
 after `warmup`). The card name and power limit are read in the same run. Writes nothing to the tree.
+
+--modes default,skip runs each workload in both modes in the same process, the runs alternating between them, and prints one
+line per mode; skip is the skip-covered mode (DESIGN.md section 18). A skip line adds the skip stats of the gapped stage and
+whether every skip-mode alignment's score, records, strand and intervals are among the default mode's (subset_of_default,
+when both modes ran). --skip-covered is --modes skip.
 """
 import argparse
 import json
@@ -55,17 +61,37 @@ def assembly(seed=2026, target_len=10_000_000, pieces=80):
     return [target], [np.concatenate(parts)], dict(pieces=pieces, reverse_complemented=rc)
 
 
-def run(name, targets, queries, steps, warmup, extra):
+def key(r):
+    return tuple(int(r[f]) for f in ("score", "target_record", "query_record", "strand", "query_begin", "query_end", "target_begin",
+                                     "target_end"))
+
+
+def run(name, targets, queries, steps, warmup, extra, modes=("default",)):
     from genomeworks_b200 import cudaextender as ce
-    al = ce.GenomeAligner()
+    aligners = {m: ce.GenomeAligner(skip_covered=m == "skip") for m in modes}
     for _ in range(warmup):
-        al.run(targets, queries)
-    t0 = time.perf_counter()
+        for al in aligners.values():
+            al.run(targets, queries)
+    wall = dict.fromkeys(modes, 0.0)
+    out = {}
     for _ in range(steps):
-        rec, _ = al.run(targets, queries)
-    wall = (time.perf_counter() - t0) / steps
-    ms, counts = al.last_stats()
-    al.close()
+        for m, al in aligners.items():
+            t0 = time.perf_counter()
+            out[m] = al.run(targets, queries)[0]
+            wall[m] += (time.perf_counter() - t0) / steps
+    for m, al in aligners.items():
+        ms, counts = al.last_stats()
+        more = dict(extra, mode=m)
+        if m == "skip":
+            more["skip_stats"] = al.last_skip_stats()
+            if "default" in out:
+                default = {key(r) for r in out["default"]}
+                more["subset_of_default"] = all(key(r) in default for r in out["skip"])
+        al.close()
+        line(name, targets, queries, steps, warmup, out[m], wall[m], ms, counts, more)
+
+
+def line(name, targets, queries, steps, warmup, rec, wall, ms, counts, extra):
     gpu, power = card()
     seeding = ms["count"] + ms["write"]
     line = dict(workload=name, target_bases=int(sum(len(t) for t in targets)), query_bases=int(sum(len(q) for q in queries)),
@@ -83,7 +109,12 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--workloads", default="sample,assembly")
+    ap.add_argument("--modes", default="default")
+    ap.add_argument("--skip-covered", action="store_true")
     a = ap.parse_args()
+    modes = ["skip"] if a.skip_covered else a.modes.split(",")
+    if set(modes) - {"default", "skip"}:
+        sys.exit("modes are default and skip")
     import torch
     if not torch.cuda.is_available():
         sys.exit("bench_genome_aligner.py needs a CUDA device")
@@ -91,10 +122,10 @@ def main():
         if w == "sample":
             import extender_libs as xl
             seq, _, _ = xl.sample()
-            run("sample", [seq], [seq], a.steps, a.warmup, {})
+            run("sample", [seq], [seq], a.steps, a.warmup, {}, modes)
         elif w == "assembly":
             t, q, extra = assembly()
-            run("assembly", t, q, a.steps, a.warmup, extra)
+            run("assembly", t, q, a.steps, a.warmup, extra, modes)
         else:
             sys.exit("unknown workload " + w)
 

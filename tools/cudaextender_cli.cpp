@@ -51,6 +51,9 @@ namespace
             seeds per ungapped extension block [33554432]; the output does not depend on it
         -b, --traceback-budget
             device bytes for gapped tracebacks [1073741824]; an alignment whose traceback needs more is written without cg:Z:
+        --skip-covered
+            do not extend an anchor that lies on an alignment already found for the same record pair and strand; anchors
+            are taken by ungapped score, highest first
         -h, --help
             this text
         -v, --version
@@ -137,12 +140,14 @@ int main(int argc, char* argv[])
         {"ydrop", required_argument, 0, 'y'},           {"gap-open", required_argument, 0, 'o'},
         {"gap-extend", required_argument, 0, 'e'},      {"gapped-threshold", required_argument, 0, 'g'},
         {"block-size", required_argument, 0, 'B'},      {"traceback-budget", required_argument, 0, 'b'},
+        {"skip-covered", no_argument, 0, 257},
         {"version", no_argument, 0, 'v'},               {"help", no_argument, 0, 'h'},
         {0, 0, 0, 0},
     };
     gwb200_genome_aligner_params p;
     gwb200_genome_aligner_default_params(&p);
     const int64_t i32 = INT32_MAX;
+    bool skip_covered = false;
     int argument      = 0;
     while ((argument = getopt_long(argc, argv, "s:x:T:y:o:e:g:B:b:vh", options, nullptr)) != -1)
     {
@@ -165,6 +170,7 @@ int main(int argc, char* argv[])
             break;
         }
         case 256: p.transition = 0; break;
+        case 257: skip_covered = true; break;
         case 'x': p.xdrop = static_cast<int32_t>(to_int(optarg, "xdrop", 0, i32)); break;
         case 'T': p.ssp_threshold = static_cast<int32_t>(to_int(optarg, "ssp-threshold", -i32 - 1, i32)); break;
         case 'y': p.ydrop = static_cast<int32_t>(to_int(optarg, "ydrop", 0, 1 << 28)); break;
@@ -193,6 +199,8 @@ int main(int argc, char* argv[])
     gwb200_genome_aligner* a = nullptr;
     if (gwb200_genome_aligner_create(&a, &p, nullptr, 0, nullptr, nullptr, nullptr) != 0)
         fail("could not create the aligner (is there a CUDA device?)");
+    if (skip_covered && gwb200_genome_aligner_set_skip_covered(a, 1, 0) != 0)
+        fail("could not set the skip-covered mode");
     const int rc = gwb200_genome_aligner_run(a, tcodes.data(), toff.data(), static_cast<int32_t>(targets.size()), qcodes.data(), qoff.data(),
                                              static_cast<int32_t>(queries.size()));
     if (rc != 0)
