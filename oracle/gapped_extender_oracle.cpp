@@ -41,6 +41,7 @@ struct SideResult
     int64_t best = 0, bi = 0, bd = 0;
     int64_t live = 0;
     int64_t storage = 0; // traceback bytes: 4 per 8 cells of each anti-diagonal's range, 8 per anti-diagonal, 1 per op
+    int64_t width   = 1; // widest cell range hi - lo + 1 of any anti-diagonal formed, the last one (with no live cell) included
     std::string ops;     // traceback order (from the best cell back to (0, 0))
 };
 
@@ -86,6 +87,7 @@ SideResult side(const Params& p, int64_t q0, int64_t t0, bool left, bool trace)
         }
         if (lo > hi)
             break;
+        r.width = std::max(r.width, hi - lo + 1);
         cur.assign(static_cast<size_t>(hi - lo + 1), Cell{kNegInf, kNegInf, kNegInf});
         std::vector<uint8_t> nib(cur.size(), 0);
         int64_t mx = kNegInf;
@@ -224,10 +226,10 @@ struct Run
 
 extern "C" {
 
-// One side: out = {best, best_i, best_d, live cells, storage bytes}; ops (traceback order, NUL-terminated) when ops != NULL and
-// it has room for best_d + 1 bytes.
-int oracle_gapped_side(const int8_t* q, int64_t qlen, const int8_t* t, int64_t tlen, const int32_t* sub, int64_t o, int64_t e, int64_t y,
-                       int64_t q0, int64_t t0, int32_t left, int64_t* out, char* ops, int64_t ops_cap)
+// oracle_gapped_side with a sixth output, out[5] = the widest range of the side (SideResult::width). A separate entry point, so
+// callers of the five-output form keep their buffers.
+int oracle_gapped_side_width(const int8_t* q, int64_t qlen, const int8_t* t, int64_t tlen, const int32_t* sub, int64_t o, int64_t e,
+                             int64_t y, int64_t q0, int64_t t0, int32_t left, int64_t* out, char* ops, int64_t ops_cap)
 {
     const Params p{q, t, qlen, tlen, sub, o, e, y};
     const SideResult r = side(p, q0, t0, left != 0, ops != nullptr);
@@ -236,6 +238,7 @@ int oracle_gapped_side(const int8_t* q, int64_t qlen, const int8_t* t, int64_t t
     out[2] = r.bd;
     out[3] = r.live;
     out[4] = r.storage;
+    out[5] = r.width;
     if (ops)
     {
         if (static_cast<int64_t>(r.ops.size()) + 1 > ops_cap)
@@ -243,6 +246,17 @@ int oracle_gapped_side(const int8_t* q, int64_t qlen, const int8_t* t, int64_t t
         std::memcpy(ops, r.ops.c_str(), r.ops.size() + 1);
     }
     return 0;
+}
+
+// One side: out = {best, best_i, best_d, live cells, storage bytes}; ops (traceback order, NUL-terminated) when ops != NULL and
+// it has room for best_d + 1 bytes.
+int oracle_gapped_side(const int8_t* q, int64_t qlen, const int8_t* t, int64_t tlen, const int32_t* sub, int64_t o, int64_t e, int64_t y,
+                       int64_t q0, int64_t t0, int32_t left, int64_t* out, char* ops, int64_t ops_cap)
+{
+    int64_t all[6];
+    const int rc = oracle_gapped_side_width(q, qlen, t, tlen, sub, o, e, y, q0, t0, left, all, ops, ops_cap);
+    std::memcpy(out, all, 5 * sizeof(int64_t));
+    return rc;
 }
 
 // Every anchor: both sides, then the threshold, the duplicate rule and, where the alignment's traceback storage fits `budget`,

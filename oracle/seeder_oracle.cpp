@@ -4,9 +4,12 @@
 // LASTZ's 12-of-19 seed 1110100110010101111. The window ending at position p (p >= 18) is used when its 19 codes are all in
 // 0..3. Query position q and target position t hit when their windows agree at the 12 care positions, or (transition != 0)
 // differ there by exactly one transition, code xor 2. Order: q ascending; within q, the exact hits, then the transitions at care
-// position 0, 1, ... 11; within each, t ascending. Target windows are bucketed by a counting sort on the full 12-code key.
+// position 0, 1, ... 11; within each, t ascending. Target windows are sorted by (12-code key, position) and each key's run is
+// found by a binary search.
 
+#include <algorithm>
 #include <cstdint>
+#include <utility>
 #include <vector>
 
 namespace
@@ -48,22 +51,13 @@ extern "C" {
 // the first `cap` seeds. Returns the total.
 int64_t oracle_seeder_run(const int8_t* query, int64_t qlen, const int8_t* target, int64_t tlen, int32_t transition, uint32_t* out, int64_t cap)
 {
-    const uint32_t keys = 1u << 24;
-    std::vector<uint32_t> start(static_cast<size_t>(keys) + 1, 0);
-    std::vector<uint32_t> tkey(static_cast<size_t>(tlen), keys);
+    // the target windows as (key, position) pairs, sorted: each key's positions in ascending order
+    std::vector<std::pair<uint32_t, uint32_t>> index;
     int codes[12];
     for (int64_t t = 0; t < tlen; ++t)
         if (window(target, tlen, t, codes))
-        {
-            tkey[t] = pack(codes);
-            start[tkey[t] + 1]++;
-        }
-    for (uint32_t k = 0; k < keys; ++k)
-        start[k + 1] += start[k];
-    std::vector<uint32_t> fill(start.begin(), start.end() - 1), bucket(start[keys]);
-    for (int64_t t = 0; t < tlen; ++t)
-        if (tkey[t] < keys)
-            bucket[fill[tkey[t]]++] = static_cast<uint32_t>(t);
+            index.emplace_back(pack(codes), static_cast<uint32_t>(t));
+    std::sort(index.begin(), index.end());
 
     int64_t n = 0;
     for (int64_t q = 0; q < qlen; ++q)
@@ -78,11 +72,12 @@ int64_t oracle_seeder_run(const int8_t* query, int64_t qlen, const int8_t* targe
             if (v >= 0)
                 c[v] ^= 2;
             const uint32_t key = pack(c);
-            for (uint32_t i = start[key]; i < start[key + 1]; ++i, ++n)
+            auto it = std::lower_bound(index.begin(), index.end(), std::make_pair(key, uint32_t(0)));
+            for (; it != index.end() && it->first == key; ++it, ++n)
                 if (n < cap)
                 {
                     out[2 * n]     = static_cast<uint32_t>(q);
-                    out[2 * n + 1] = bucket[i];
+                    out[2 * n + 1] = it->second;
                 }
         }
     }

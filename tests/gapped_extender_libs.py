@@ -25,6 +25,8 @@ def oracle():
     return load("liboracle_gapped_extender.so", {
         "oracle_gapped_side": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
                                          C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_char_p, C.c_int64]),
+        "oracle_gapped_side_width": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64,
+                                               C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_char_p, C.c_int64]),
         "oracle_gapped_run": (C.c_void_p, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
                                            C.c_int64, C.c_void_p, C.c_int64, C.c_int64]),
         "oracle_gapped_count": (C.c_int64, [C.c_void_p]),
@@ -40,14 +42,15 @@ def _arrays(query, target, matrix):
 
 
 def oracle_side(query, target, matrix, o, e, y, q0, t0, left, trace=True):
-    """-> dict(best, i, d, live, storage, ops) of one side; ops in traceback order (best cell back to (0, 0))."""
+    """-> dict(best, i, d, live, storage, width, ops) of one side; ops in traceback order (best cell back to (0, 0)); width is
+    the widest cell range hi - lo + 1 of any anti-diagonal the side formed, as the device sizes its rings by it."""
     q, t, m = _arrays(query, target, matrix)
-    out = np.zeros(5, dtype=np.int64)
+    out = np.zeros(6, dtype=np.int64)
     cap = len(q) + len(t) + 2
     buf = C.create_string_buffer(cap) if trace else None
-    rc = oracle().oracle_gapped_side(ptr(q), len(q), ptr(t), len(t), ptr(m), o, e, y, q0, t0, int(left), ptr(out), buf, cap)
+    rc = oracle().oracle_gapped_side_width(ptr(q), len(q), ptr(t), len(t), ptr(m), o, e, y, q0, t0, int(left), ptr(out), buf, cap)
     assert rc == 0
-    r = dict(zip(("best", "i", "d", "live", "storage"), (int(v) for v in out)))
+    r = dict(zip(("best", "i", "d", "live", "storage", "width"), (int(v) for v in out)))
     r["ops"] = buf.value.decode() if trace else None
     return r
 
