@@ -65,6 +65,16 @@ class GenomeAlignerParams(C.Structure):
     ]
 
 
+class ChainStats(C.Structure):
+    """gwb200_chain_stats."""
+    _fields_ = [
+        ("ssps_in", C.c_int64),
+        ("ssps_chained", C.c_int64),
+        ("pairs", C.c_int64),
+        ("chain_ms", C.c_double),
+    ]
+
+
 class IndexArrays(C.Structure):
     """gwb200_index_arrays: the six arrays of a cudamapper index and its scalars."""
     _fields_ = [
@@ -296,6 +306,17 @@ def lib():
     L.gwb200_genome_aligner_last_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     L.gwb200_genome_aligner_set_skip_covered.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
     L.gwb200_genome_aligner_last_skip_stats.argtypes = [C.c_void_p, C.c_void_p]
+    L.gwb200_genome_aligner_set_chain.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
+    L.gwb200_genome_aligner_last_chain_stats.argtypes = [C.c_void_p, C.POINTER(ChainStats)]
+    L.gwb200_ssp_chainer_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_ssp_chainer_destroy.argtypes = [C.c_void_p]
+    L.gwb200_ssp_chainer_destroy.restype = None
+    L.gwb200_ssp_chainer_chain_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
+    for name in ("sync", "num_chained"):
+        getattr(L, "gwb200_ssp_chainer_" + name).argtypes = [C.c_void_p]
+    L.gwb200_ssp_chainer_get_chain.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]
+    L.gwb200_ssp_chainer_get_dp.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gwb200_ssp_chainer_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
     L.gwb200_index_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int64, C.c_uint32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_double, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     L.gwb200_index_wait.argtypes = [C.c_void_p]

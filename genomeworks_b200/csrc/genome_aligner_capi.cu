@@ -7,9 +7,11 @@
 // them gives exactly the result of one extender call over all the seeds. The unique segments go to the gapped extender on the
 // device; their alignments come back with CIGARs, and the host maps minus-strand query intervals to forward coordinates and
 // counts the PAF columns. In skip-covered mode (DESIGN.md section 18) the gapped extender of each pair and strand runs the
-// sequential rule in its own coordinates.
+// sequential rule in its own coordinates. With chaining on (DESIGN.md section 19) the unique segments of each pair and strand
+// are chained first, and only the chain's segments go to the gapped extender.
 
 #include "../../include/gwb200.h"
+#include "chain_internal.cuh"
 #include "common.cuh"
 #include "extender_internal.cuh"
 
@@ -75,11 +77,14 @@ struct gwb200_genome_aligner
     gwb200_seeder* seeder          = nullptr;
     gwb200_extender* ungapped      = nullptr;
     gwb200_gapped_extender* gapped = nullptr;
+    gwb200_ssp_chainer* chainer    = nullptr;
+    bool chain_on        = false;
+    int32_t chain_pen[2] = {0, 0}; // diagonal, anti-diagonal
 
     DevBuf<int8_t> target_d{&hooks}, query_d{&hooks}, rc_d{&hooks};
     const int8_t* target_h = nullptr; // the host codes of the indexed target record
     DevBuf<SeedRec> seeds_d{&hooks};
-    DevBuf<SspRec> kept_d{&hooks}, spare_d{&hooks}, ssps_d{&hooks};
+    DevBuf<SspRec> kept_d{&hooks}, spare_d{&hooks}, ssps_d{&hooks}, chained_d{&hooks};
     DevBuf<int32_t> counts_d{&hooks}; // [0] kept segments, [1] unique segments
     DevBuf<unsigned long long> examined_d{&hooks};
     EventTimer timer;
@@ -92,12 +97,14 @@ struct gwb200_genome_aligner
     float stage_ms[kStages] = {};
     int64_t n_seeds = 0, n_ssps = 0;
     int64_t skip_stats[5] = {}; // the gapped extender's, summed over pairs and strands
+    gwb200_chain_stats chain_stats{};
 
     ~gwb200_genome_aligner()
     {
         gwb200_seeder_destroy(seeder);
         gwb200_extender_destroy(ungapped);
         gwb200_gapped_extender_destroy(gapped);
+        gwb200_ssp_chainer_destroy(chainer);
     }
 };
 
@@ -209,9 +216,31 @@ int align_pair(gwb200_genome_aligner* a, int32_t ti, int32_t qi, int32_t strand,
     if (n_ssps == 0)
         return 0;
 
+    // chain: only the chain's segments, in ascending index, go on
+    const SspRec* anchors = a->ssps_d.p;
+    int32_t n_anchors     = n_ssps;
+    if (a->chain_on)
+    {
+        if (!a->chained_d.ensure(n_ssps))
+            return bad_alloc();
+        if (const int rc = chain::chain_ssps(a->chainer, a->ssps_d.p, n_ssps, a->chain_pen[0], a->chain_pen[1], a->chained_d.p))
+            return rc;
+        n_anchors = gwb200_ssp_chainer_num_chained(a->chainer);
+        float ms  = -1.f;
+        if (n_anchors < 0)
+            return n_anchors;
+        if (const int rc = gwb200_ssp_chainer_last_ms(a->chainer, &ms))
+            return rc;
+        anchors = a->chained_d.p;
+        a->chain_stats.ssps_in += n_ssps;
+        a->chain_stats.ssps_chained += n_anchors;
+        a->chain_stats.pairs += 1;
+        a->chain_stats.chain_ms += std::max(0.f, ms);
+    }
+
     // gapped
     int rc = gwb200_gapped_extender_extend_ssps_device(a->gapped, query_dev, static_cast<int32_t>(qlen), a->target_d.p, static_cast<int32_t>(tlen),
-                                                       p.gapped_threshold, a->ssps_d.p, n_ssps);
+                                                       p.gapped_threshold, anchors, n_anchors);
     if (rc == 0)
         rc = gwb200_gapped_extender_sync(a->gapped);
     if (rc != 0)
@@ -303,6 +332,7 @@ void clear(gwb200_genome_aligner* a)
     std::fill(a->stage_ms, a->stage_ms + kStages, 0.f);
     a->n_seeds = a->n_ssps = 0;
     std::fill(a->skip_stats, a->skip_stats + 5, int64_t(0));
+    a->chain_stats = gwb200_chain_stats{};
 }
 
 int run(gwb200_genome_aligner* a, const int8_t* targets, const int64_t* toff, int32_t nt, const int8_t* queries, const int64_t* qoff, int32_t nq)
@@ -399,6 +429,8 @@ int gwb200_genome_aligner_create(gwb200_genome_aligner** out, const gwb200_genom
     if (rc == 0)
         rc = gwb200_extender_create_with_allocator(&a->ungapped, params->score_matrix, 64, params->xdrop, 0, stream, device_id, alloc_fn, free_fn,
                                                    user);
+    if (rc == 0)
+        rc = gwb200_ssp_chainer_create(&a->chainer, stream, device_id, alloc_fn, free_fn, user);
     if (rc == 0)
         rc = gwb200_gapped_extender_create_with_allocator(&a->gapped, params->score_matrix, 64, params->gap_open, params->gap_extend,
                                                           params->ydrop, params->traceback_budget, stream, device_id, alloc_fn, free_fn, user);
@@ -509,6 +541,28 @@ int gwb200_genome_aligner_last_skip_stats(const gwb200_genome_aligner* a, int64_
     if (!a->ready)
         return set_error(GWB200_E_RUNTIME, "no finished run: call gwb200_genome_aligner_run first");
     std::copy(a->skip_stats, a->skip_stats + 5, out);
+    return 0;
+}
+
+int gwb200_genome_aligner_set_chain(gwb200_genome_aligner* a, int32_t on, int32_t diag_penalty, int32_t anti_penalty)
+{
+    if (diag_penalty < 0 || diag_penalty > (1 << 20) || anti_penalty < 0 || anti_penalty > (1 << 20))
+        return GWB200_EXT_INVALID_INPUT;
+    if (!a)
+        return set_error(GWB200_E_INVALID_ARGUMENT, "null genome aligner");
+    a->chain_on     = on != 0;
+    a->chain_pen[0] = diag_penalty;
+    a->chain_pen[1] = anti_penalty;
+    return GWB200_EXT_SUCCESS;
+}
+
+int gwb200_genome_aligner_last_chain_stats(const gwb200_genome_aligner* a, gwb200_chain_stats* out)
+{
+    if (!a || !out)
+        return set_error(GWB200_E_INVALID_ARGUMENT, "null argument");
+    if (!a->ready)
+        return set_error(GWB200_E_RUNTIME, "no finished run: call gwb200_genome_aligner_run first");
+    *out = a->chain_stats;
     return 0;
 }
 

@@ -8,7 +8,8 @@
 Sequences are int8 arrays of codes or str (encoded with encode_sequence); seed pairs are a structured array with named
 `query` and `target` fields (SEED_DTYPE), so the CSV's target-first column order cannot be confused with the record order.
 create_gapped_extender (GappedXDrop) turns anchors into gapped alignments with CIGARs. create_seeder (Seeder) makes the seed
-pairs of two sequences, and align_genomes / format_paf run seeding and both extension stages over two sets of records.
+pairs of two sequences, create_ssp_chainer (SspChainer) finds the highest-scoring colinear chain of scored segment pairs,
+and align_genomes / format_paf run seeding, both extension stages and, optionally, chaining over two sets of records.
 There is no CPU fallback: without a CUDA device create_extender and create_gapped_extender raise.
 """
 import ctypes as C
@@ -365,6 +366,116 @@ def create_seeder(transition=True, stream=None, device_id=0, allocator=None):
     return Seeder(transition, stream, device_id, allocator)
 
 
+# Chaining (DESIGN.md section 19): the highest-scoring colinear chain of scored segment pairs.
+MAX_CHAIN_PENALTY = 1 << 20
+CHAIN_STATS = ("ssps_in", "ssps_chained", "pairs", "chain_ms")
+
+
+def _penalty(name, v):
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+        raise TypeError("%s must be an integer" % name)
+    if not 0 <= int(v) <= MAX_CHAIN_PENALTY:
+        raise ValueError("%s must lie in [0, 2^20]" % name)
+    return int(v)
+
+
+def _chain_arg(chain):
+    """None or False: no chaining; True: penalties (0, 0); (D, A): those penalties, checked before any device work."""
+    if chain is None or chain is False:
+        return None
+    if chain is True:
+        return 0, 0
+    if isinstance(chain, (tuple, list)) and len(chain) == 2:
+        return _penalty("the diagonal penalty", chain[0]), _penalty("the anti-diagonal penalty", chain[1])
+    raise TypeError("chain must be None, True or a (diag_penalty, anti_penalty) pair")
+
+
+class SspChainer:
+    """The chaining DP of DESIGN.md section 19 on the device: chain(ssps) returns the SSP indices of the highest-scoring colinear
+    chain, in ascending order, and its score; get_dp() returns f and p of every SSP."""
+
+    def __init__(self, stream=None, device_id=0, allocator=None):
+        self._args = CallArgs(stream, allocator)
+        self._device = device_id
+        self._h = C.c_void_p()
+        self._n = 0
+        check(lib().gwb200_ssp_chainer_create(C.byref(self._h), self._args.stream, C.c_int32(device_id), *self._args.mem))
+
+    def chain(self, ssps, n=None, diag_penalty=0, anti_penalty=0):
+        """ssps: an SSP_DTYPE array (copied to the device), a CUDA tensor of n x 4 int32 values (query, target, length, score) or
+        a device address (then n is required). Blocking. Penalties outside [0, 2^20], n < 0 or a length below -1 raise
+        ValueError."""
+        D = _penalty("diag_penalty", diag_penalty)
+        A = _penalty("anti_penalty", anti_penalty)
+        keep = None
+        if isinstance(ssps, np.ndarray):
+            import torch
+            rows = np.ascontiguousarray(ssps, dtype=SSP_DTYPE).view(np.int32).reshape(-1, 4)
+            n = len(rows) if n is None else n
+            if not 0 <= int(n) <= len(rows):
+                raise ValueError("n must lie in [0, %d]" % len(rows))
+            keep = torch.from_numpy(rows).to("cuda:%d" % self._device)
+            addr = keep.data_ptr() if keep.numel() else 0
+        elif hasattr(ssps, "data_ptr"):
+            n = ssps.shape[0] if n is None else n
+            addr = ssps.data_ptr() if ssps.numel() else 0
+        else:
+            if n is None:
+                raise ValueError("n is required with a device address")
+            addr = int(ssps or 0)
+        if int(n) < 0:
+            raise ValueError("n must be >= 0")
+        rc = check(lib().gwb200_ssp_chainer_chain_device(self._h, C.c_void_p(addr), C.c_int32(int(n)), C.c_int32(D), C.c_int32(A)))
+        if rc == invalid_input:
+            raise ValueError("invalid chain arguments")
+        if rc == invalid_operation:
+            raise RuntimeError("a chain call is pending")
+        rc = check(lib().gwb200_ssp_chainer_sync(self._h))
+        del keep
+        if rc == invalid_input:
+            raise ValueError("an SSP length is below -1")
+        self._n = int(n)
+        return self.get_chain()
+
+    def get_chain(self):
+        """(int32 SSP indices of the chain in ascending order, score) of the last call."""
+        m = check(lib().gwb200_ssp_chainer_num_chained(self._h))
+        idx = np.zeros(m, dtype=np.int32)
+        score = C.c_int64()
+        check(lib().gwb200_ssp_chainer_get_chain(self._h, idx.ctypes.data_as(C.c_void_p), C.byref(score)))
+        return idx, score.value
+
+    def get_dp(self):
+        """(f as int64, p as int32, -1 for none) of every SSP of the last call, by SSP index."""
+        check(lib().gwb200_ssp_chainer_num_chained(self._h))
+        f = np.zeros(self._n, dtype=np.int64)
+        p = np.zeros(self._n, dtype=np.int32)
+        check(lib().gwb200_ssp_chainer_get_dp(self._h, f.ctypes.data_as(C.c_void_p), p.ctypes.data_as(C.c_void_p)))
+        return f, p
+
+    def last_ms(self):
+        """Device ms of the last call."""
+        ms = C.c_float()
+        check(lib().gwb200_ssp_chainer_last_ms(self._h, C.byref(ms)))
+        return ms.value
+
+    def close(self):
+        if self._h:
+            lib().gwb200_ssp_chainer_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def create_ssp_chainer(stream=None, device_id=0, allocator=None):
+    """An SspChainer. Without a CUDA device this raises RuntimeError."""
+    return SspChainer(stream, device_id, allocator)
+
+
 # The genome-to-genome aligner (DESIGN.md section 17): seeds, blocked ungapped extension and gapped extension of every
 # (target record, query record) pair on one or both strands.
 GENOME_DTYPE = np.dtype([("score", np.int64), ("target_record", np.int32), ("query_record", np.int32), ("strand", np.int32),
@@ -395,11 +506,12 @@ def _records(seqs):
 class GenomeAligner:
     """The aligner with fixed parameters; run(targets, queries) aligns every query record against every target record."""
 
-    def __init__(self, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, round_anchors=0, **params):
+    def __init__(self, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, round_anchors=0, chain=None, **params):
         from ._lib import GenomeAlignerParams
         if strand not in STRANDS:
             raise ValueError("strand must be one of %s" % ", ".join(STRANDS))
         skip = _skip_args(skip_covered, round_anchors)
+        penalties = _chain_arg(chain)
         p = default_genome_params()
         unknown = set(params) - set(p)
         if unknown:
@@ -424,6 +536,13 @@ class GenomeAligner:
         check(rc)
         if skip[0]:
             check(lib().gwb200_genome_aligner_set_skip_covered(self._h, C.c_int32(skip[0]), C.c_int32(skip[1])))
+        if penalties is not None:
+            self.set_chain(penalties)
+
+    def set_chain(self, chain):
+        """Chaining for later runs (DESIGN.md section 19): None or False turns it off, True or (D, A) turns it on."""
+        penalties = _chain_arg(chain)
+        check(lib().gwb200_genome_aligner_set_chain(self._h, int(penalties is not None), *(C.c_int32(v) for v in penalties or (0, 0))))
 
     def run(self, targets, queries):
         """-> (GENOME_DTYPE records, CIGAR strings, '' where has_cigar is 0). Blocking."""
@@ -457,6 +576,14 @@ class GenomeAligner:
         check(lib().gwb200_genome_aligner_last_skip_stats(self._h, out.ctypes.data_as(C.c_void_p)))
         return dict(zip(SKIP_STATS, (int(v) for v in out)))
 
+    def last_chain_stats(self):
+        """Of the last run, summed over every pair and strand: {ssps_in, ssps_chained, pairs, chain_ms} (all zero without
+        chaining; DESIGN.md section 19)."""
+        from ._lib import ChainStats
+        st = ChainStats()
+        check(lib().gwb200_genome_aligner_last_chain_stats(self._h, C.byref(st)))
+        return {name: getattr(st, name) for name in CHAIN_STATS}
+
     def close(self):
         if self._h:
             lib().gwb200_genome_aligner_destroy(self._h)
@@ -469,14 +596,15 @@ class GenomeAligner:
             pass
 
 
-def align_genomes(targets, queries, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, **params):
+def align_genomes(targets, queries, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, chain=None, **params):
     """Aligns every query record against every target record on the plus strand, the minus strand or both. targets and queries
     are lists of sequences (str or int8 codes). Keyword parameters override gwb200_genome_aligner_default_params: score_matrix,
     xdrop, ssp_threshold, gap_open, gap_extend, ydrop, gapped_threshold, transition, block_size, traceback_budget. Returns
     (GENOME_DTYPE records, CIGAR strings); query coordinates are forward for both strands and minus-strand CIGARs read the
     target forward. Bad parameters raise ValueError before any device work. skip_covered=True does not extend the anchors that
-    lie on an alignment kept earlier for the same pair and strand (DESIGN.md section 18)."""
-    al = GenomeAligner(strand, stream, device_id, allocator, skip_covered, **params)
+    lie on an alignment kept earlier for the same pair and strand (DESIGN.md section 18). chain=True or (D, A) extends only the
+    SSPs of the highest-scoring colinear chain of each pair and strand (DESIGN.md section 19)."""
+    al = GenomeAligner(strand, stream, device_id, allocator, skip_covered, chain=chain, **params)
     try:
         return al.run(targets, queries)
     finally:

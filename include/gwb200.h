@@ -500,6 +500,36 @@ int gwb200_seeder_sync(gwb200_seeder* seeder);
 int gwb200_seeder_last_ms(gwb200_seeder* seeder, float* index_ms, float* count_ms, float* write_ms);
 
 /* ------------------------------------------------------------------------------------------------
+ * cudaextender, chaining stage (DESIGN.md section 19): the highest-scoring colinear chain of n ScoredSegmentPair records. The
+ * reference has no counterpart.
+ * SSP k covers query [q_k, q_k + L_k] and target [t_k, t_k + L_k] (L = -1 covers nothing). i precedes j iff
+ * t_i + L_i < t_j and q_i + L_i < q_j (when two L = -1 segments share a start, only the smaller index precedes the other).
+ * With dq = q_j - q_i - L_i - 1 and dt = t_j - t_i - L_i - 1, pen(i, j) = D |dt - dq| + A (dq + dt), and
+ * f(j) = s_j + max(0, max over i preceding j of f(i) - pen(i, j)); p(j) = the smallest i attaining a maximum > 0, else -1.
+ * The chain ends at the smallest j with the largest f and follows p; its score is that f. All arithmetic is int64.
+ * ---------------------------------------------------------------------------------------------- */
+
+typedef struct gwb200_ssp_chainer gwb200_ssp_chainer; /* opaque */
+
+/* Device buffers come from the caller's allocator when alloc_fn and free_fn are given. GWB200_E_CUDA without a device. */
+int gwb200_ssp_chainer_create(gwb200_ssp_chainer** out, void* stream, int32_t device_id, gwb200_device_alloc_fn alloc_fn,
+                              gwb200_device_free_fn free_fn, void* user);
+void gwb200_ssp_chainer_destroy(gwb200_ssp_chainer* chainer);
+/* Chains d_ssps[0, n) (device memory, valid until sync) with diagonal penalty D and anti-diagonal penalty A, enqueued on the
+ * chainer's stream without waiting. invalid_input, before any device work, for D or A outside [0, 2^20], n < 0 or NULL data;
+ * invalid_operation while a call is pending. */
+int gwb200_ssp_chainer_chain_device(gwb200_ssp_chainer* chainer, const void* d_ssps, int32_t n, int32_t diag_penalty, int32_t anti_penalty);
+/* Blocking: finishes the pending call. invalid_operation when none is pending; invalid_input when an SSP length is below -1. */
+int gwb200_ssp_chainer_sync(gwb200_ssp_chainer* chainer);
+/* After sync(): the chain's length; its SSP indices in ascending order (num_chained entries) and its score (0 for n = 0); f[n]
+ * and p[n] by SSP index (get_dp returns n). Without a finished call => GWB200_E_RUNTIME. */
+int32_t gwb200_ssp_chainer_num_chained(const gwb200_ssp_chainer* chainer);
+int gwb200_ssp_chainer_get_chain(const gwb200_ssp_chainer* chainer, int32_t* indices, int64_t* score);
+int gwb200_ssp_chainer_get_dp(const gwb200_ssp_chainer* chainer, int64_t* f, int32_t* p);
+/* Device ms of the last finished call (CUDA events; -1 when not available). */
+int gwb200_ssp_chainer_last_ms(const gwb200_ssp_chainer* chainer, float* ms);
+
+/* ------------------------------------------------------------------------------------------------
  * cudaextender, genome-to-genome aligner (DESIGN.md section 17): every (target record, query record) pair on the plus strand,
  * the minus strand (the query reverse-complemented on the device) or both: seeds (above), ungapped X-drop extension of every
  * seed in blocks of at most block_size seeds with one sort and unique over all kept segments (identical to one extender call
@@ -572,6 +602,20 @@ int gwb200_genome_aligner_last_stats(const gwb200_genome_aligner* aligner, float
 int gwb200_genome_aligner_set_skip_covered(gwb200_genome_aligner* aligner, int32_t on, int32_t round_anchors);
 /* gwb200_gapped_extender_last_skip_stats of the last run, summed over every pair and strand. */
 int gwb200_genome_aligner_last_skip_stats(const gwb200_genome_aligner* aligner, int64_t* out);
+/* Chaining (DESIGN.md section 19), off by default; it holds for later runs until turned off. With on != 0, the unique SSPs of
+ * each (pair, strand) are chained (gwb200_ssp_chainer_*, penalties D and A) in the strand's own coordinates, and only the
+ * chain's SSPs, in ascending index, go to the gapped stage. invalid_input for D or A outside [0, 2^20], before the handle is
+ * looked at. */
+int gwb200_genome_aligner_set_chain(gwb200_genome_aligner* aligner, int32_t on, int32_t diag_penalty, int32_t anti_penalty);
+typedef struct gwb200_chain_stats
+{
+    int64_t ssps_in;      /* unique SSPs given to the chainer */
+    int64_t ssps_chained; /* SSPs on the chains, given to the gapped stage */
+    int64_t pairs;        /* (pair, strand)s chained: those with at least one SSP */
+    double chain_ms;      /* device ms of the chainer */
+} gwb200_chain_stats;
+/* Of the last run, summed over every pair and strand (all zero with chaining off). */
+int gwb200_genome_aligner_last_chain_stats(const gwb200_genome_aligner* aligner, gwb200_chain_stats* out);
 
 /* ------------------------------------------------------------------------------------------------
  * cudamapper (minimizer index)

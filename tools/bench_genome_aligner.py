@@ -1,8 +1,8 @@
 """Genome aligner benchmark: one JSON line per workload, with the aligner's defaults (both strands, transitions, the sample
 matrix, LASTZ-style gapped parameters, blocks of 2^25 seeds).
 
-    python tools/bench_genome_aligner.py [--steps K] [--warmup W] [--workloads sample,assembly] [--modes default,skip]
-                                         [--skip-covered]
+    python tools/bench_genome_aligner.py [--steps K] [--warmup W] [--workloads sample,assembly]
+                                         [--modes default,skip,chain,chain+skip] [--skip-covered]
 
 Workloads:
   sample    the golden sample (one 250 kb record) against itself;
@@ -18,7 +18,8 @@ after `warmup`). The card name and power limit are read in the same run. Writes 
 --modes default,skip runs each workload in both modes in the same process, the runs alternating between them, and prints one
 line per mode; skip is the skip-covered mode (DESIGN.md section 18). A skip line adds the skip stats of the gapped stage and
 whether every skip-mode alignment's score, records, strand and intervals are among the default mode's (subset_of_default,
-when both modes ran). --skip-covered is --modes skip.
+when both modes ran). --skip-covered is --modes skip. chain is chaining with zero penalties (DESIGN.md section 19) and
+chain+skip chaining in skip-covered mode; their lines add the chain stats (SSPs in, SSPs chained, pairs, chain ms).
 """
 import argparse
 import json
@@ -68,7 +69,7 @@ def key(r):
 
 def run(name, targets, queries, steps, warmup, extra, modes=("default",)):
     from genomeworks_b200 import cudaextender as ce
-    aligners = {m: ce.GenomeAligner(skip_covered=m == "skip") for m in modes}
+    aligners = {m: ce.GenomeAligner(skip_covered=m in ("skip", "chain+skip"), chain=m in ("chain", "chain+skip")) for m in modes}
     for _ in range(warmup):
         for al in aligners.values():
             al.run(targets, queries)
@@ -82,6 +83,8 @@ def run(name, targets, queries, steps, warmup, extra, modes=("default",)):
     for m, al in aligners.items():
         ms, counts = al.last_stats()
         more = dict(extra, mode=m)
+        if m in ("chain", "chain+skip"):
+            more["chain_stats"] = al.last_chain_stats()
         if m == "skip":
             more["skip_stats"] = al.last_skip_stats()
             if "default" in out:
@@ -113,8 +116,8 @@ def main():
     ap.add_argument("--skip-covered", action="store_true")
     a = ap.parse_args()
     modes = ["skip"] if a.skip_covered else a.modes.split(",")
-    if set(modes) - {"default", "skip"}:
-        sys.exit("modes are default and skip")
+    if set(modes) - {"default", "skip", "chain", "chain+skip"}:
+        sys.exit("modes are default, skip, chain and chain+skip")
     import torch
     if not torch.cuda.is_available():
         sys.exit("bench_genome_aligner.py needs a CUDA device")

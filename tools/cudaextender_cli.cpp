@@ -1,6 +1,6 @@
 // gw-b200: the `cudaextender` command line tool: `cudaextender [options] target.fa query.fa > out.paf`. Every query record is
 // aligned against every target record by the library's genome aligner (gwb200_genome_aligner_*, DESIGN.md section 17): spaced
-// seeds, ungapped X-drop extension, gapped extension with CIGARs, on one or both strands. The files are read in file order
+// seeds, ungapped X-drop extension, optional chaining, gapped extension with CIGARs, on one or both strands. The files are read in file order
 // (FASTA or FASTQ) and encoded as cudaextender::encode_sequence does. Every check happens before the first CUDA call.
 #include <gwb200.h>
 
@@ -54,6 +54,9 @@ namespace
         --skip-covered
             do not extend an anchor that lies on an alignment already found for the same record pair and strand; anchors
             are taken by ungapped score, highest first
+        --chain[=D,A]
+            extend only the highest-scoring colinear chain of ungapped segments of each record pair and strand; D and A
+            are the diagonal and anti-diagonal gap penalties of the chain, each in [0, 1048576] [0,0]
         -h, --help
             this text
         -v, --version
@@ -140,14 +143,15 @@ int main(int argc, char* argv[])
         {"ydrop", required_argument, 0, 'y'},           {"gap-open", required_argument, 0, 'o'},
         {"gap-extend", required_argument, 0, 'e'},      {"gapped-threshold", required_argument, 0, 'g'},
         {"block-size", required_argument, 0, 'B'},      {"traceback-budget", required_argument, 0, 'b'},
-        {"skip-covered", no_argument, 0, 257},
+        {"skip-covered", no_argument, 0, 257},          {"chain", optional_argument, 0, 258},
         {"version", no_argument, 0, 'v'},               {"help", no_argument, 0, 'h'},
         {0, 0, 0, 0},
     };
     gwb200_genome_aligner_params p;
     gwb200_genome_aligner_default_params(&p);
     const int64_t i32 = INT32_MAX;
-    bool skip_covered = false;
+    bool skip_covered = false, chain = false;
+    int32_t chain_pen[2] = {0, 0};
     int argument      = 0;
     while ((argument = getopt_long(argc, argv, "s:x:T:y:o:e:g:B:b:vh", options, nullptr)) != -1)
     {
@@ -171,6 +175,22 @@ int main(int argc, char* argv[])
         }
         case 256: p.transition = 0; break;
         case 257: skip_covered = true; break;
+        case 258:
+        {
+            chain = true;
+            if (!optarg)
+                break;
+            const std::string s = optarg;
+            const size_t comma  = s.find(',');
+            if (comma == std::string::npos)
+            {
+                std::cerr << "ERROR: chain takes D,A (two integers in [0, 1048576]), not '" << s << "'" << std::endl;
+                std::exit(1);
+            }
+            chain_pen[0] = static_cast<int32_t>(to_int(s.substr(0, comma).c_str(), "chain's diagonal penalty", 0, 1 << 20));
+            chain_pen[1] = static_cast<int32_t>(to_int(s.substr(comma + 1).c_str(), "chain's anti-diagonal penalty", 0, 1 << 20));
+            break;
+        }
         case 'x': p.xdrop = static_cast<int32_t>(to_int(optarg, "xdrop", 0, i32)); break;
         case 'T': p.ssp_threshold = static_cast<int32_t>(to_int(optarg, "ssp-threshold", -i32 - 1, i32)); break;
         case 'y': p.ydrop = static_cast<int32_t>(to_int(optarg, "ydrop", 0, 1 << 28)); break;
@@ -201,6 +221,8 @@ int main(int argc, char* argv[])
         fail("could not create the aligner (is there a CUDA device?)");
     if (skip_covered && gwb200_genome_aligner_set_skip_covered(a, 1, 0) != 0)
         fail("could not set the skip-covered mode");
+    if (chain && gwb200_genome_aligner_set_chain(a, 1, chain_pen[0], chain_pen[1]) != 0)
+        fail("could not set chaining");
     const int rc = gwb200_genome_aligner_run(a, tcodes.data(), toff.data(), static_cast<int32_t>(targets.size()), qcodes.data(), qoff.data(),
                                              static_cast<int32_t>(queries.size()));
     if (rc != 0)
