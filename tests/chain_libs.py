@@ -1,19 +1,15 @@
 """Checkers of the SSP chainer (DESIGN.md section 19): ctypes bindings for its CPU oracle (oracle/liboracle_chain.so), a plain-
-Python restatement of the contract that pins the oracle, SSP set generators, and the genome aligner's chained composition --
-seeder oracle, ungapped oracle, chain oracle, then the gapped oracle or the skip-covered oracle. TEST INFRASTRUCTURE ONLY."""
+Python restatement of the contract that pins the oracle, SSP set generators and a check of the contract's equations on the
+device. TEST INFRASTRUCTURE ONLY."""
 import ctypes as C
 import functools
 import sys
 
 import numpy as np
 
-import extender_libs as xl
-import gapped_extender_libs as gl
-import gapped_skip_libs as sk
-import seeder_libs as sl
 from checker_lib import load, ptr
+from extender_libs import SSP_DTYPE
 
-SSP_DTYPE = np.dtype([("query", np.uint32), ("target", np.uint32), ("length", np.int32), ("score", np.int32)])
 MAX_PENALTY = 1 << 20
 
 
@@ -176,62 +172,3 @@ def check_contract_on_device(ssps, D, A, f, p, chain, score, rows_per_step=256, 
     while p[walk[-1]] >= 0:
         walk.append(int(p[walk[-1]]))
     assert score == int(f[e]) and np.array_equal(np.sort(walk), chain)
-
-
-_ungapped = {}
-
-
-def ungapped_ssps(qs, target, p):
-    """The unique SSPs of the seeder and ungapped oracles, kept for the process: the chained compositions of one test share
-    them."""
-    key = (qs.tobytes(), np.asarray(target, np.int8).tobytes(), bool(p["transition"]), np.asarray(p["matrix"]).tobytes(), p["xdrop"],
-           p["ssp_threshold"])
-    if key not in _ungapped:
-        seeds = sl.oracle_run(qs, target, p["transition"])
-        _ungapped[key] = xl.oracle_run(qs, target, p["matrix"], p["xdrop"], False, p["ssp_threshold"], seeds)
-    return _ungapped[key]
-
-
-def _strand_records(ti, qi, strand, query, target, p, penalties, skip):
-    """(records as tuples, CIGARs, SSPs in, SSPs chained) of one pair and strand with chaining."""
-    qs = sl.reverse_complement(query) if strand else np.asarray(query, np.int8)
-    ssps = ungapped_ssps(qs, target, p)
-    if len(ssps) == 0:
-        return [], [], 0, 0
-    kept = ssps[chain_indices(oracle_run(ssps, *penalties))]
-    anchors = sk.ssp_anchors(kept)
-    args = (qs, target, p["matrix"], p["gap_open"], p["gap_extend"], p["ydrop"], p["gapped_threshold"], anchors)
-    budget = p.get("traceback_budget", 1 << 30)
-    if skip:
-        rec, cigars, _, _ = sk.skip_run(*args, sk.ssp_order(kept), budget)
-    else:
-        rec, cigars, _ = gl.oracle_run(*args, budget)
-    rows, L = [], len(query)
-    for r, cg in zip(rec, cigars):
-        qb, qe = int(r["query_begin"]), int(r["query_end"])
-        if strand:
-            qb, qe = L - qe, L - qb
-        matches, block = sl.paf_columns(cg, qs, target, int(r["query_begin"]), int(r["target_begin"]), bool(r["has_cigar"]), qe - qb,
-                                        int(r["target_end"]) - int(r["target_begin"]))
-        rows.append((int(r["score"]), ti, qi, strand, int(r["has_cigar"]), qb, qe, int(r["target_begin"]), int(r["target_end"]),
-                     matches, block))
-    return rows, cigars, len(ssps), len(kept)
-
-
-def aligner_chain_oracle(targets, queries, strand="both", chain=(0, 0), skip=False, **params):
-    """(record tuples in the engine's order, CIGARs, {ssps_in, ssps_chained, pairs}) of align_genomes(..., chain=chain,
-    skip_covered=skip)."""
-    p = dict(sl.DEFAULTS)
-    p.update(params)
-    strands = {"plus": [0], "minus": [1], "both": [0, 1]}[strand]
-    rows, cigars, stats = [], [], {"ssps_in": 0, "ssps_chained": 0, "pairs": 0}
-    for ti, t in enumerate(targets):
-        for qi, q in enumerate(queries):
-            for s in strands:
-                r, c, n_in, n_kept = _strand_records(ti, qi, s, np.asarray(q, np.int8), np.asarray(t, np.int8), p, chain, skip)
-                rows += r
-                cigars += c
-                stats["ssps_in"] += n_in
-                stats["ssps_chained"] += n_kept
-                stats["pairs"] += int(n_in > 0)
-    return rows, cigars, stats

@@ -1,6 +1,7 @@
 """The one loader of the checkers the tests compare the engine against: the CPU restatements oracle/lib*.so (built by
 oracle/Makefile) and the libraries of the unmodified reference under oracle/_ref/, and the gzip JSON fixtures under
-tests/golden/. TEST INFRASTRUCTURE ONLY."""
+tests/golden/. Also the one device allocator the GPU tests hand to the engines to check that their memory balances. TEST
+INFRASTRUCTURE ONLY."""
 import ctypes as C
 import gzip
 import json
@@ -48,3 +49,27 @@ def write_fixture(path, obj):
     os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
     with gzip.GzipFile(path, "wb", mtime=0) as f:
         f.write(json.dumps(obj, sort_keys=True).encode())
+
+
+class CountingAllocator:
+    """Device memory from torch's caching allocator; counts the requests, keeps the size of each block outstanding, checks
+    that a block is freed with its size, and can refuse its n-th request."""
+
+    def __init__(self, refuse=None):
+        import torch
+        self.torch = torch
+        self.live = {}
+        self.calls = 0
+        self.refuse = refuse
+
+    def alloc(self, n):
+        self.calls += 1
+        if self.calls == self.refuse:
+            return 0
+        p = self.torch.cuda.caching_allocator_alloc(int(n))
+        self.live[p] = n
+        return p
+
+    def free(self, p, n):
+        assert self.live.pop(p) == n
+        self.torch.cuda.caching_allocator_delete(p)

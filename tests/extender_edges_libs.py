@@ -3,6 +3,7 @@ device): asymmetric scoring schemes, ranges of exact widths at the chunk and rin
 lane or chunk boundary. TEST INFRASTRUCTURE ONLY."""
 import numpy as np
 
+import extender_libs as xl
 import gapped_extender_libs as gl
 
 # Only (target A, query C) scores positive: reading the matrix as sub[query * 8 + target] changes every result built on it.
@@ -35,7 +36,7 @@ def with_odd_bytes(codes, rng, rate=0.05):
 # Widths at which the device changes path: one chunk (256) or two, the shared ring (512) or one rerun (C = 2048), one rerun
 # or two (C = 8192), two reruns or three (C = 32768).
 WIDTH_EDGES = (256, 257, 512, 513, 2048, 2049, 8192, 8193)
-WIDTH_PARAMS = (gl.SIMPLE_MATRIX, 1, 1, 1 << 28)  # matrix, open, extend, y-drop: at this y-drop no cell is ever pruned
+WIDTH_PARAMS = (xl.SIMPLE_MATRIX, 1, 1, 1 << 28)  # matrix, open, extend, y-drop: at this y-drop no cell is ever pruned
 WIDTH_PAIRS = ((8193, 256), (257, 8192), (2049, 512), (513, 2048))  # (left width, right width) of one anchor each
 
 
@@ -60,7 +61,7 @@ def width_case(seed=61):
 # lie on either side of a lane boundary (p = 6, 14), of a chunk boundary (p = 254) and of a chunk boundary past the shared
 # ring (p = 510). The smaller i wins: query [0, p + 1), target [0, p + 2).
 TIE_PS = (6, 14, 254, 510)
-TIE_PARAMS = (gl.SIMPLE_MATRIX, 1, 1, 1 << 20)
+TIE_PARAMS = (xl.SIMPLE_MATRIX, 1, 1, 1 << 20)
 
 
 def tie_case(p):

@@ -135,6 +135,12 @@ def synthetic_cases():
     ]
 
 
+def ssps_on_device(ssps):
+    """An SSP_DTYPE array as the n x 4 int32 CUDA tensor (query, target, length, score) the device-pointer calls take."""
+    import torch
+    return torch.from_numpy(np.ascontiguousarray(ssps, dtype=SSP_DTYPE).view(np.int32).reshape(-1, 4).copy()).cuda()
+
+
 def ssp_rows(a):
     return [[int(r["query"]), int(r["target"]), int(r["length"]), int(r["score"])] for r in a]
 

@@ -1,24 +1,28 @@
-"""Checkers of the gapped extender: ctypes bindings for the CPU oracle (oracle/liboracle_gapped_extender.so), a separate CIGAR
-re-scorer, an unpruned numpy DP and the parameters the tests share. TEST INFRASTRUCTURE ONLY."""
+"""Checkers of the gapped extender: ctypes bindings for the CPU oracle (oracle/liboracle_gapped_extender.so), the anchor rule
+for scored segment pairs, a separate CIGAR re-scorer, an unpruned numpy DP and the parameters and inputs the tests share. TEST
+INFRASTRUCTURE ONLY."""
 import ctypes as C
 import re
 
 import numpy as np
 
+import extender_libs as xl
 from checker_lib import load, ptr
 
-ANCHOR_DTYPE = np.dtype([("query", np.uint32), ("target", np.uint32)])
+ANCHOR_DTYPE = xl.SEED_DTYPE
 GAPPED_DTYPE = np.dtype([("score", np.int64), ("anchor", np.int32), ("has_cigar", np.int32), ("query_begin", np.uint32),
                          ("query_end", np.uint32), ("target_begin", np.uint32), ("target_end", np.uint32)])
 FIELDS = GAPPED_DTYPE.names
 
 # LASTZ-style gapped parameters over the ungapped extender's sample matrix
 LASTZ_OPEN, LASTZ_EXTEND, LASTZ_YDROP, LASTZ_THRESHOLD = 400, 30, 9400, 3000
-# +10 / -10 among A/C/G/T, -20 against the other codes
-SIMPLE_MATRIX = np.full((8, 8), -20, dtype=np.int32)
-SIMPLE_MATRIX[:4, :4] = -10
-np.fill_diagonal(SIMPLE_MATRIX[:4, :4], 10)
-SIMPLE_MATRIX = SIMPLE_MATRIX.ravel()
+# the functions that read a run's results out of its handle, in this oracle and in the skip-covered one built on it
+FETCH_SIGNATURES = {
+    "oracle_gapped_count": (C.c_int64, [C.c_void_p]),
+    "oracle_gapped_live": (C.c_int64, [C.c_void_p]),
+    "oracle_gapped_text_bytes": (C.c_int64, [C.c_void_p]),
+    "oracle_gapped_fetch": (None, [C.c_void_p, C.c_void_p, C.c_char_p, C.c_void_p]),
+    "oracle_gapped_free": (None, [C.c_void_p])}
 
 
 def oracle():
@@ -29,11 +33,7 @@ def oracle():
                                                C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_char_p, C.c_int64]),
         "oracle_gapped_run": (C.c_void_p, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
                                            C.c_int64, C.c_void_p, C.c_int64, C.c_int64]),
-        "oracle_gapped_count": (C.c_int64, [C.c_void_p]),
-        "oracle_gapped_live": (C.c_int64, [C.c_void_p]),
-        "oracle_gapped_text_bytes": (C.c_int64, [C.c_void_p]),
-        "oracle_gapped_fetch": (None, [C.c_void_p, C.c_void_p, C.c_char_p, C.c_void_p]),
-        "oracle_gapped_free": (None, [C.c_void_p])})
+        **FETCH_SIGNATURES})
 
 
 def _arrays(query, target, matrix):
@@ -60,7 +60,11 @@ def oracle_run(query, target, matrix, o, e, y, threshold, anchors, budget=1 << 6
     q, t, m = _arrays(query, target, matrix)
     a = np.ascontiguousarray(anchors, dtype=ANCHOR_DTYPE)
     L = oracle()
-    h = L.oracle_gapped_run(ptr(q), len(q), ptr(t), len(t), ptr(m), o, e, y, threshold, ptr(a), len(a), budget)
+    return _fetch(L, L.oracle_gapped_run(ptr(q), len(q), ptr(t), len(t), ptr(m), o, e, y, threshold, ptr(a), len(a), budget))
+
+
+def _fetch(L, h):
+    """(GAPPED_DTYPE records, CIGAR strings, live cells) of the run handle h of library L, which is then freed."""
     try:
         n = L.oracle_gapped_count(h)
         rec = np.zeros(n, dtype=GAPPED_DTYPE)
@@ -72,6 +76,20 @@ def oracle_run(query, target, matrix, o, e, y, threshold, anchors, budget=1 << 6
         return rec, [raw[offsets[k]:offsets[k + 1]] for k in range(n)], L.oracle_gapped_live(h)
     finally:
         L.oracle_gapped_free(h)
+
+
+def ssp_anchors(ssps):
+    """The anchor of each scored segment pair (SSP_DTYPE): its midpoint, as the device takes it."""
+    a = np.zeros(len(ssps), dtype=ANCHOR_DTYPE)
+    a["query"] = ssps["query"] + ssps["length"] // 2
+    a["target"] = ssps["target"] + ssps["length"] // 2
+    return a
+
+
+def synthetic(n=300, seed=21):
+    """(target, query, seeds) of a 30 kb homologous pair at 15 % divergence with n seeds, 30 % of them spurious."""
+    from genomeworks_b200 import synth
+    return synth.extender_workload(30000, 0.15, n, 0.3, seed=seed)
 
 
 def rows(rec):

@@ -1,18 +1,15 @@
-"""Checkers of the seeder and the genome aligner: ctypes bindings for the seeder's CPU oracle (oracle/liboracle_seeder.so), the
-golden seed file, and the aligner's oracle composition -- seeder oracle, ungapped extender oracle over all seeds, gapped
-extender oracle, numpy reverse complement and coordinate mapping, and the PAF rules restated here. TEST INFRASTRUCTURE ONLY."""
+"""Checkers of the seeder: ctypes bindings for its CPU oracle (oracle/liboracle_seeder.so), the golden seed file, and the
+sequence helpers the seeder's and the genome aligner's tests share: reverse complement, mutation, a rearranged pair and FASTA
+text. TEST INFRASTRUCTURE ONLY."""
 import ctypes as C
 import gzip
 import os
-import re
 
 import numpy as np
 
 import extender_libs as xl
-import gapped_extender_libs as gl
 from checker_lib import load, ptr
 
-SEED_DTYPE = np.dtype([("query", np.uint32), ("target", np.uint32)])
 PATTERN = "1110100110010101111"
 CARE = [i for i, c in enumerate(PATTERN) if c == "1"]
 
@@ -23,11 +20,11 @@ def oracle():
 
 
 def oracle_run(query, target, transition=True):
-    """The seed pairs of query against target in the engine's global order (SEED_DTYPE)."""
+    """The seed pairs of query against target in the engine's global order (xl.SEED_DTYPE)."""
     q, t = np.ascontiguousarray(query, np.int8), np.ascontiguousarray(target, np.int8)
     L = oracle()
     n = L.oracle_seeder_run(ptr(q), len(q), ptr(t), len(t), int(bool(transition)), None, 0)
-    out = np.zeros(n, dtype=SEED_DTYPE)
+    out = np.zeros(n, dtype=xl.SEED_DTYPE)
     L.oracle_seeder_run(ptr(q), len(q), ptr(t), len(t), int(bool(transition)), ptr(out), n)
     return out
 
@@ -52,81 +49,6 @@ def reverse_complement(codes):
     m = (c >= 0) & (c < 4)
     c[m] = 3 - c[m]
     return c
-
-
-# the aligner's defaults (gwb200_genome_aligner_default_params)
-DEFAULTS = dict(matrix=xl.SAMPLE_MATRIX, xdrop=xl.SAMPLE_XDROP, ssp_threshold=xl.SAMPLE_THRESHOLD, gap_open=gl.LASTZ_OPEN,
-                gap_extend=gl.LASTZ_EXTEND, ydrop=gl.LASTZ_YDROP, gapped_threshold=gl.LASTZ_THRESHOLD, transition=True)
-
-
-def _strand_records(ti, qi, strand, query, target, p):
-    """(records as tuples, CIGARs) of one pair and strand: the oracle composition."""
-    qs = reverse_complement(query) if strand else np.asarray(query, np.int8)
-    seeds = oracle_run(qs, target, p["transition"])
-    ssps = xl.oracle_run(qs, target, p["matrix"], p["xdrop"], False, p["ssp_threshold"], seeds)
-    if len(ssps) == 0:
-        return [], [], []
-    anchors = np.zeros(len(ssps), dtype=gl.ANCHOR_DTYPE)
-    anchors["query"] = ssps["query"] + ssps["length"] // 2
-    anchors["target"] = ssps["target"] + ssps["length"] // 2
-    rec, cigars, _ = gl.oracle_run(qs, target, p["matrix"], p["gap_open"], p["gap_extend"], p["ydrop"], p["gapped_threshold"], anchors)
-    rows, at = [], []
-    L = len(query)
-    for r, cg in zip(rec, cigars):
-        qb, qe = int(r["query_begin"]), int(r["query_end"])
-        if strand:
-            qb, qe = L - qe, L - qb
-        matches, block = paf_columns(cg, qs, target, int(r["query_begin"]), int(r["target_begin"]), bool(r["has_cigar"]),
-                                     qe - qb, int(r["target_end"]) - int(r["target_begin"]))
-        rows.append((int(r["score"]), ti, qi, strand, int(r["has_cigar"]), qb, qe, int(r["target_begin"]), int(r["target_end"]),
-                     matches, block))
-        a = anchors[int(r["anchor"])]
-        at.append((int(a["query"]), int(a["target"])))
-    return rows, cigars, at
-
-
-def paf_columns(cigar, qcodes, tcodes, qb, tb, has_cigar, qspan, tspan):
-    """PAF columns 10 and 11: M positions with equal codes in 0..3, and the sum of M, I and D lengths; without a CIGAR 0 and the
-    larger span."""
-    if not has_cigar:
-        return 0, max(qspan, tspan)
-    matches = block = 0
-    for n, op in re.findall(r"(\d+)([MID])", cigar):
-        n = int(n)
-        block += n
-        if op == "M":
-            a = np.asarray(qcodes[qb:qb + n])
-            b = np.asarray(tcodes[tb:tb + n])
-            matches += int(((a == b) & (a >= 0) & (a < 4)).sum())
-            qb += n
-            tb += n
-        elif op == "I":
-            qb += n
-        else:
-            tb += n
-    return matches, block
-
-
-def aligner_oracle(targets, queries, strand="both", **params):
-    """(record tuples in the engine's order, CIGARs, the anchor of each in its strand's coordinates) of align_genomes over the
-    records (int8 codes)."""
-    p = dict(DEFAULTS)
-    p.update(params)
-    strands = {"plus": [0], "minus": [1], "both": [0, 1]}[strand]
-    rows, cigars, anchors = [], [], []
-    for ti, t in enumerate(targets):
-        for qi, q in enumerate(queries):
-            for s in strands:
-                r, c, a = _strand_records(ti, qi, s, np.asarray(q, np.int8), np.asarray(t, np.int8), p)
-                rows += r
-                cigars += c
-                anchors += a
-    return rows, cigars, anchors
-
-
-def engine_rows(rec):
-    return [tuple(int(r[f]) for f in ("score", "target_record", "query_record", "strand", "has_cigar", "query_begin", "query_end",
-                                      "target_begin", "target_end", "matches", "block_length")) for r in rec]
 
 
 def mutate(codes, rate, rng):
@@ -163,15 +85,3 @@ def rearranged_pair(seed, n=30000, rate=0.04):
 def text(codes):
     """FASTA text that encode_sequence maps back to `codes` (0-3 ACGT, 4 lowercase a, 5 N)."""
     return "".join("ACGTaN"[int(c)] for c in codes)
-
-
-def paf_oracle(rows, cigars, target_names, target_lengths, query_names, query_lengths):
-    lines = []
-    for r, cg in zip(rows, cigars):
-        score, ti, qi, strand, has_cigar, qb, qe, tb, te, matches, block = r
-        cols = [query_names[qi], query_lengths[qi], qb, qe, "-" if strand else "+", target_names[ti], target_lengths[ti], tb, te,
-                matches, block, 255, "AS:i:%d" % score]
-        if has_cigar:
-            cols.append("cg:Z:" + cg)
-        lines.append("\t".join(str(c) for c in cols) + "\n")
-    return "".join(lines)

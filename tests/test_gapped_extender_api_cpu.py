@@ -7,6 +7,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import extender_libs as xl
 import gapped_extender_libs as gl
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -22,7 +23,7 @@ def L():
 
 
 def create(L, mat=None, dim=64, o=400, e=30, y=9400, budget=1 << 20):
-    m = np.ascontiguousarray(gl.SIMPLE_MATRIX if mat is None else mat, dtype=np.int32)
+    m = np.ascontiguousarray(xl.SIMPLE_MATRIX if mat is None else mat, dtype=np.int32)
     h = C.c_void_p()
     rc = L.gwb200_gapped_extender_create(C.byref(h), m.ctypes.data_as(C.c_void_p), dim, o, e, y, budget, None, 0)
     return rc, h
@@ -36,7 +37,7 @@ def test_create_rejects_parameters_out_of_range(L, kw):
 
 @pytest.mark.parametrize("v", [-(1 << 24) - 1, (1 << 24) + 1])
 def test_create_rejects_matrix_entries_out_of_range(L, v):
-    m = gl.SIMPLE_MATRIX.copy()
+    m = xl.SIMPLE_MATRIX.copy()
     m[9] = v
     assert create(L, mat=m)[0] == INVALID_INPUT
 
@@ -44,7 +45,7 @@ def test_create_rejects_matrix_entries_out_of_range(L, v):
 def test_create_rejects_a_null_matrix_and_a_null_handle(L):
     h = C.c_void_p()
     assert L.gwb200_gapped_extender_create(C.byref(h), None, 64, 1, 1, 1, 0, None, 0) == INVALID_INPUT
-    m = np.ascontiguousarray(gl.SIMPLE_MATRIX)
+    m = np.ascontiguousarray(xl.SIMPLE_MATRIX)
     assert L.gwb200_gapped_extender_create(None, m.ctypes.data_as(C.c_void_p), 64, 1, 1, 1, 0, None, 0) == -1
 
 
@@ -101,7 +102,7 @@ def test_null_handle_calls(L):
                                 dict(score_matrix=np.full(64, 1 << 25, dtype=np.int64))])
 def test_python_rejects_parameters_before_any_device_work(L, kw):
     from genomeworks_b200 import cudaextender as ce
-    args = dict(score_matrix=gl.SIMPLE_MATRIX, gap_open=400, gap_extend=30, ydrop=9400)
+    args = dict(score_matrix=xl.SIMPLE_MATRIX, gap_open=400, gap_extend=30, ydrop=9400)
     args.update(kw)
     with pytest.raises(ValueError):
         ce.create_gapped_extender(**args)
@@ -113,7 +114,7 @@ def test_python_without_a_device_raises(L):
         pytest.skip("a device is present")
     from genomeworks_b200 import cudaextender as ce
     with pytest.raises(RuntimeError):
-        ce.create_gapped_extender(gl.SIMPLE_MATRIX, 400, 30, 9400)
+        ce.create_gapped_extender(xl.SIMPLE_MATRIX, 400, 30, 9400)
 
 
 def test_header_compiles_warning_free_as_cpp14(tmp_path):

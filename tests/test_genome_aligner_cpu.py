@@ -7,6 +7,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import genome_aligner_libs as ga
 import seeder_libs as sl
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -23,10 +24,10 @@ def ce():
 
 def test_defaults_are_the_tests_parameters(ce):
     p = ce.default_genome_params()
-    assert np.array_equal(p["score_matrix"], sl.DEFAULTS["matrix"])
+    assert np.array_equal(p["score_matrix"], ga.DEFAULTS["matrix"])
     assert (p["xdrop"], p["ssp_threshold"], p["gap_open"], p["gap_extend"], p["ydrop"], p["gapped_threshold"], p["transition"]) == (
-        sl.DEFAULTS["xdrop"], sl.DEFAULTS["ssp_threshold"], sl.DEFAULTS["gap_open"], sl.DEFAULTS["gap_extend"], sl.DEFAULTS["ydrop"],
-        sl.DEFAULTS["gapped_threshold"], 1)
+        ga.DEFAULTS["xdrop"], ga.DEFAULTS["ssp_threshold"], ga.DEFAULTS["gap_open"], ga.DEFAULTS["gap_extend"], ga.DEFAULTS["ydrop"],
+        ga.DEFAULTS["gapped_threshold"], 1)
     assert p["block_size"] == 1 << 25 and p["strand"] == 3 and p["traceback_budget"] == 1 << 30
 
 
@@ -38,7 +39,7 @@ def test_bad_parameters_raise_before_device_work(ce, bad):
 
 
 def test_bad_matrix_strand_and_names(ce):
-    m = np.array(sl.DEFAULTS["matrix"]).copy()
+    m = np.array(ga.DEFAULTS["matrix"]).copy()
     m[3] = (1 << 24) + 1
     with pytest.raises(ValueError):
         ce.align_genomes(["A"], ["A"], score_matrix=m)
@@ -94,7 +95,7 @@ def test_format_paf_minus_strand(ce):
         "read1\t100\t60\t90\t-\tchrB\t2000\t200\t229\t27\t31\t255\tAS:i:4500\tcg:Z:10M1I9M2D10M",
         "read2\t50\t5\t40\t+\tchrA\t1000\t7\t42\t35\t35\t255\tAS:i:3100\tcg:Z:35M",
         "read1\t100\t0\t100\t-\tchrA\t1000\t300\t380\t0\t100\t255\tAS:i:9000"]
-    assert got == sl.paf_oracle(sl.engine_rows(rec), cigars, ["chrA", "chrB"], [1000, 2000], ["read1", "read2"], [100, 50])
+    assert got == ga.paf_oracle(ga.engine_rows(rec), cigars, ["chrA", "chrB"], [1000, 2000], ["read1", "read2"], [100, 50])
 
 
 def test_paf_columns_on_the_reverse_complement():
@@ -103,9 +104,9 @@ def test_paf_columns_on_the_reverse_complement():
     assert rc.tolist() == [2, 3, 3, 4, 0, 1, 2, 3]
     t = np.array([2, 3, 3, 4, 0, 1, 2, 2], dtype=np.int8)
     # 8M over rc: equal at 0, 1, 2, 4, 5, 6 (4 equals 4 but is not in 0..3)
-    assert sl.paf_columns("8M", rc, t, 0, 0, True, 8, 8) == (6, 8)
-    assert sl.paf_columns("3M1I2M1D2M", rc, t, 0, 0, True, 8, 8) == (4, 9)
-    assert sl.paf_columns("", rc, t, 0, 0, False, 8, 6) == (0, 8)
+    assert ga.paf_columns("8M", rc, t, 0, 0, True, 8, 8) == (6, 8)
+    assert ga.paf_columns("3M1I2M1D2M", rc, t, 0, 0, True, 8, 8) == (4, 9)
+    assert ga.paf_columns("", rc, t, 0, 0, False, 8, 6) == (0, 8)
 
 
 def cli(args):

@@ -3,18 +3,17 @@ sample's SSPs, random sets on both sides of the tile sizes, ladders, anti-diagon
 genome aligner with chaining against the oracle composition (seeder -> ungapped -> chain -> gapped or skip-covered), in records,
 CIGARs, PAF and chain stats."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import chain_libs as cl
 import extender_libs as xl
+import genome_aligner_libs as ga
 import seeder_libs as sl
+from checker_lib import CountingAllocator
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 K = 1024  # chain_kernels.cuh kTile
 TOP = 1 << 20
 PENALTIES = [(0, 0), (1, 1), (TOP, TOP), (1, 0), (0, TOP)]
@@ -120,23 +119,6 @@ def test_ties_planted_across_tile_boundaries(chainer):
     assert np.array_equal(got["chain"], np.arange(K + 7))
 
 
-class CountingAllocator:
-    def __init__(self):
-        import torch
-        self.torch = torch
-        self.live = {}
-        self.calls = 0
-
-    def alloc(self, n):
-        t = self.torch.empty(int(n), dtype=self.torch.uint8, device="cuda")
-        self.live[t.data_ptr()] = t
-        self.calls += 1
-        return t.data_ptr()
-
-    def free(self, p, n):
-        del self.live[p]
-
-
 def test_reuse_with_a_stream_and_an_allocator(ce):
     import torch
     from genomeworks_b200._lib import lib
@@ -149,7 +131,7 @@ def test_reuse_with_a_stream_and_an_allocator(ce):
         assert_oracle(run(c, ssps, 1, 2), ssps, 1, 2)
     # a CUDA tensor and a raw device address give the same result
     ssps = cl.random_ssps(rng, 900, span=3000)
-    dev = torch.from_numpy(ssps.view(np.int32).reshape(-1, 4).copy()).cuda()
+    dev = xl.ssps_on_device(ssps)
     torch.cuda.synchronize()
     want = cl.oracle_run(ssps)
     assert np.array_equal(c.chain(dev)[0], cl.chain_indices(want))
@@ -177,85 +159,52 @@ def test_reuse_with_a_stream_and_an_allocator(ce):
     assert alloc.live == {}
 
 
-def check_aligner(ce, targets, queries, strand="both", chain=(0, 0), skip=False, **params):
-    al = ce.GenomeAligner(strand, chain=chain, skip_covered=skip, **params)
-    rec, cigars = al.run(targets, queries)
-    stats = al.last_chain_stats()
-    al.close()
-    rows, want_cigars, want_stats = cl.aligner_chain_oracle(targets, queries, strand, tuple(chain), skip,
-                                                            **{k: v for k, v in params.items() if k != "block_size"})
-    assert sl.engine_rows(rec) == rows
-    assert cigars == want_cigars
-    assert {k: stats[k] for k in want_stats} == want_stats
-    assert (stats["chain_ms"] > 0) == (want_stats["pairs"] > 0)
-    return rec, cigars, stats
-
-
-def records_case():
-    rng = np.random.default_rng(17)
-    shared = rng.integers(0, 4, 6000).astype(np.int8)
-    targets = [np.concatenate([rng.integers(0, 4, 2000).astype(np.int8), shared[:3000]]),
-               rng.integers(0, 4, 4000).astype(np.int8),
-               np.concatenate([sl.reverse_complement(shared[2500:]), rng.integers(0, 4, 1000).astype(np.int8)])]
-    queries = [sl.mutate(shared, 0.03, rng), np.concatenate([rng.integers(0, 4, 500).astype(np.int8), sl.mutate(targets[1][1000:3000], 0.05, rng)])]
-    queries[1][100:140] = 5
-    return targets, queries
-
-
 def test_aligner_golden_sample(ce):
     seq, _, _ = xl.sample()
     default, _ = ce.align_genomes([seq], [seq])
     for chain in ((0, 0), (2, 1)):
-        rec, _, stats = check_aligner(ce, [seq], [seq], chain=chain)
+        rec, _, _, stats = ga.check_aligner(ce, [seq], [seq], chain=chain)
         assert (rec["strand"] == 1).any() and stats["pairs"] == 2
         assert stats["ssps_chained"] < stats["ssps_in"] and len(rec) < len(default)
 
 
 def test_aligner_inversion_pair_and_records(ce):
     target, query, _ = sl.rearranged_pair(5)
-    rec, _, _ = check_aligner(ce, [target], [query])
+    rec = ga.check_aligner(ce, [target], [query], chain=(0, 0))[0]
     assert (rec["strand"] == 1).any()
-    targets, queries = records_case()
-    want = check_aligner(ce, targets, queries)
-    assert want[2]["pairs"] >= 3
+    targets, queries = ga.records_case()
+    want = ga.check_aligner(ce, targets, queries, chain=(0, 0))
+    assert want[3]["pairs"] >= 3
     # blocks of 7 seeds give the same output
-    got = check_aligner(ce, targets, queries, block_size=7)
-    assert sl.engine_rows(got[0]) == sl.engine_rows(want[0]) and got[1] == want[1]
+    got = ga.check_aligner(ce, targets, queries, chain=(0, 0), block_size=7)
+    assert ga.engine_rows(got[0]) == ga.engine_rows(want[0]) and got[1] == want[1]
 
 
 def test_aligner_chain_with_skip_covered(ce):
-    targets, queries = records_case()
-    check_aligner(ce, targets, queries, chain=(1, 1), skip=True)
+    targets, queries = ga.records_case()
+    ga.check_aligner(ce, targets, queries, chain=(1, 1), skip=True)
     seq, _, _ = xl.sample()
-    check_aligner(ce, [seq], [seq], skip=True)
+    ga.check_aligner(ce, [seq], [seq], chain=(0, 0), skip=True)
 
 
 def test_chained_run_then_default_run_on_one_handle(ce):
-    targets, queries = records_case()
+    targets, queries = ga.records_case()
     al = ce.GenomeAligner(chain=True)
     chained = al.run(targets, queries)
     al.set_chain(None)
     rec, cigars = al.run(targets, queries)
     assert al.last_chain_stats() == {"ssps_in": 0, "ssps_chained": 0, "pairs": 0, "chain_ms": 0.0}
     al.close()
-    rows, want_cigars, _ = sl.aligner_oracle(targets, queries)
-    assert sl.engine_rows(rec) == rows and cigars == want_cigars
+    rows, want_cigars, _, _ = ga.aligner_oracle(targets, queries)
+    assert ga.engine_rows(rec) == rows and cigars == want_cigars
     assert len(chained[0]) <= len(rec)
 
 
 def test_tool_chain_prints_the_same_paf(ce, tmp_path):
-    targets, queries = records_case()
-    tnames, qnames = ["t%d" % k for k in range(3)], ["q%d" % k for k in range(2)]
-    with open(tmp_path / "t.fa", "w") as f:
-        for n, s in zip(tnames, targets):
-            f.write(">%s\n%s\n" % (n, sl.text(s)))
-    with open(tmp_path / "q.fa", "w") as f:
-        for n, s in zip(qnames, queries):
-            f.write(">%s\n%s\n" % (n, sl.text(s)))
+    targets, queries = ga.records_case()
     for opt, chain in (("--chain", True), ("--chain=3,2", (3, 2))):
         rec, cigars = ce.align_genomes(targets, queries, chain=chain)
-        want = ce.format_paf(rec, cigars, tnames, [len(s) for s in targets], qnames, [len(s) for s in queries])
-        out = subprocess.run([os.path.join(ROOT, "build", "cudaextender"), opt, str(tmp_path / "t.fa"), str(tmp_path / "q.fa")],
-                             capture_output=True, text=True, timeout=600)
+        want = ga.tool_paf(ce, rec, cigars, targets, queries)
+        out = ga.run_tool(tmp_path, targets, queries, opt)
         assert out.returncode == 0, out.stderr
         assert out.stdout == want and want

@@ -10,6 +10,7 @@ import extender_edges_libs as el
 import extender_libs as xl
 import gapped_extender_libs as gl
 import gapped_skip_libs as sk
+import genome_aligner_libs as ga
 import seeder_libs as sl
 
 pytestmark = pytest.mark.gpu
@@ -246,14 +247,14 @@ def test_best_cell_ties_across_lane_and_chunk_boundaries(ce, p):
     check_gapped(ce, target, query, params, NO_THRESHOLD, anchors_of([(0, 0)]))
 
 
-ASYMMETRIC_TIE_MATRIX = gl.SIMPLE_MATRIX.copy()
+ASYMMETRIC_TIE_MATRIX = xl.SIMPLE_MATRIX.copy()
 ASYMMETRIC_TIE_MATRIX[[2 * 8 + 0, 3 * 8 + 1, 1 * 8 + 3, 0 * 8 + 5]] = [-3, 4, -15, 2]
 
 
 @pytest.mark.parametrize("case", el.periodic_cases(), ids=lambda c: c[0])
 def test_low_complexity_repeats_tie_everywhere(ce, case):
     _, q, t, anchors = case
-    for mat in (gl.SIMPLE_MATRIX, ASYMMETRIC_TIE_MATRIX):
+    for mat in (xl.SIMPLE_MATRIX, ASYMMETRIC_TIE_MATRIX):
         for o, e, y in ((1, 1, 3000), (0, 2, 100), (3, 0, 40)):
             check_gapped(ce, q, t, (mat, o, e, y), NO_THRESHOLD, anchors)
             check_gapped(ce, t, q, (mat, o, e, y), NO_THRESHOLD, anchors_of([(b, a) for a, b in anchors]))
@@ -266,7 +267,7 @@ def test_anchors_at_the_four_corners(ce):
     q, t = homologous(rng, 530, 500)
     m, n = len(q), len(t)
     anchors = anchors_of([(0, 0), (0, n - 1), (m - 1, 0), (m - 1, n - 1)])
-    for params in ((gl.SIMPLE_MATRIX, 5, 2, 80), (el.asymmetric_matrix(rng), 1, 0, 1000)):
+    for params in ((xl.SIMPLE_MATRIX, 5, 2, 80), (el.asymmetric_matrix(rng), 1, 0, 1000)):
         check_gapped(ce, q, t, params, NO_THRESHOLD, anchors)
         check_gapped(ce, t, q, params, NO_THRESHOLD, anchors_of([(b, a) for a, b in anchors]))
 
@@ -276,7 +277,7 @@ def test_one_base_against_a_hundred_thousand(ce):
     long = rng.integers(0, 4, 100000).astype(np.int8)
     one = np.array([2], dtype=np.int8)
     # open 1, extend 0: a gap of any length costs 1, so every side runs to the far end of the long sequence
-    for params in ((gl.SIMPLE_MATRIX, 1, 0, 50), (gl.SIMPLE_MATRIX, 5, 2, 80)):
+    for params in ((xl.SIMPLE_MATRIX, 1, 0, 50), (xl.SIMPLE_MATRIX, 5, 2, 80)):
         check_gapped(ce, one, long, params, NO_THRESHOLD, anchors_of([(0, 0), (0, 50000), (0, 99999)]))
         check_gapped(ce, long, one, params, NO_THRESHOLD, anchors_of([(0, 0), (50000, 0), (99999, 0)]))
 
@@ -288,14 +289,13 @@ def test_ssp_midpoints_on_the_last_base(ce):
     m, n = len(q), len(t)
     ssps = np.array([(m - 5, n - 5, 9, 50), (m - 4, n - 4, 7, 40), (m - 1, n - 1, 1, 10), (m - 1, n - 1, 0, 5), (0, 0, 1, 10),
                      (0, n - 1, 0, 5), (m - 1, 0, 1, 5), (m - 9, n - 5, 8, 30)], dtype=xl.SSP_DTYPE)
-    params = (gl.SIMPLE_MATRIX, 5, 2, 80)
-    anchors = sk.ssp_anchors(ssps)
+    params = (xl.SIMPLE_MATRIX, 5, 2, 80)
+    anchors = gl.ssp_anchors(ssps)
     assert (int(anchors["query"].max()), int(anchors["target"].max())) == (m - 1, n - 1)
     dq = torch.from_numpy(np.ascontiguousarray(q, np.int8)).cuda()
     dt = torch.from_numpy(np.ascontiguousarray(t, np.int8)).cuda()
-    ds = torch.from_numpy(np.ascontiguousarray(ssps).view(np.int32).reshape(-1, 4).copy()).cuda()
     x = ce.create_gapped_extender(*params)
-    assert x.extend_ssps_device(dq, dt, NO_THRESHOLD, ds, len(ssps)) == ce.success and x.sync() == ce.success
+    assert x.extend_ssps_device(dq, dt, NO_THRESHOLD, xl.ssps_on_device(ssps), len(ssps)) == ce.success and x.sync() == ce.success
     got = x.get_alignments() + (x.last_live_cells(),)
     x.close()
     assert_gapped(got, gl.oracle_run(q, t, *params, NO_THRESHOLD, anchors))
@@ -358,34 +358,14 @@ def degenerate_records(rng):
     return targets, queries
 
 
-def check_aligner(ce, targets, queries, strand, **params):
-    rec, cigars = ce.align_genomes(targets, queries, strand=strand, **params)
-    rows, want, anchors = sl.aligner_oracle(targets, queries, strand, **params)
-    assert sl.engine_rows(rec) == rows
-    assert cigars == want
-    for r, cg, (q0, t0) in zip(rec, cigars, anchors):
-        if not r["has_cigar"]:
-            continue
-        q = np.asarray(queries[r["query_record"]], np.int8)
-        qs = sl.reverse_complement(q) if r["strand"] else q
-        qb = len(q) - int(r["query_end"]) if r["strand"] else int(r["query_begin"])
-        got = gl.rescore(cg, qs, targets[r["target_record"]], sl.DEFAULTS["matrix"], gl.LASTZ_OPEN, gl.LASTZ_EXTEND, qb,
-                         int(r["target_begin"]), anchor=(q0, t0))
-        assert got == (int(r["score"]), int(r["query_end"] - r["query_begin"]), int(r["target_end"] - r["target_begin"]))
-    tn, qn = ["t%d" % k for k in range(len(targets))], ["q%d" % k for k in range(len(queries))]
-    tl, ql = [len(s) for s in targets], [len(s) for s in queries]
-    assert ce.format_paf(rec, cigars, tn, tl, qn, ql) == sl.paf_oracle(rows, want, tn, tl, qn, ql)
-    return rec
-
-
 @pytest.mark.parametrize("strand", ["both", "plus", "minus"])
 def test_aligner_on_degenerate_records(ce, strand):
     targets, queries = degenerate_records(np.random.default_rng(7000))
-    rec = check_aligner(ce, targets, queries, strand)
+    rec = ga.check_aligner(ce, targets, queries, strand)[0]
     assert len(rec) > 0
     if strand == "both":
         assert {int(v) for v in rec["strand"]} == {0, 1}
-        check_aligner(ce, targets[:3], queries, strand, transition=False)
+        ga.check_aligner(ce, targets[:3], queries, strand, transition=False)
 
 
 def test_aligner_on_forty_tiny_records_by_three(ce):
@@ -393,7 +373,7 @@ def test_aligner_on_forty_tiny_records_by_three(ce):
     shared = rng.integers(0, 4, 600).astype(np.int8)
     targets = [shared, sl.reverse_complement(shared[:300]), np.full(25, 5, np.int8)]
     queries = [shared[k * 13:k * 13 + k].copy() for k in range(40)]
-    rec = check_aligner(ce, targets, queries, "both", ssp_threshold=100, gapped_threshold=100)
+    rec = ga.check_aligner(ce, targets, queries, "both", ssp_threshold=100, gapped_threshold=100)[0]
     assert len(rec) > 0
 
 
@@ -402,7 +382,7 @@ def test_minus_strand_mapping_at_an_odd_length(ce):
     t = rng.integers(0, 4, 5001).astype(np.int8)
     q = sl.reverse_complement(t[1000:3001])  # 2001 bases, the minus strand of target[1000, 3001)
     q[[0, 1, 2, 1000, 1001, 1997, 1998, 1999, 2000]] = [4, 5, 6, 7, 4, 5, 6, 7, 4]
-    rec = check_aligner(ce, [t], [q], "both")
+    rec = ga.check_aligner(ce, [t], [q], "both")[0]
     assert len(q) % 2 == 1 and (rec["strand"] == 1).any()
 
 

@@ -7,6 +7,7 @@ import pytest
 
 import extender_libs as xl
 import gapped_extender_libs as gl
+from checker_lib import CountingAllocator
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -40,10 +41,7 @@ def assert_equal(got, want):
 
 def sample_anchors():
     seq, _, golden = xl.sample()
-    a = np.zeros(len(golden), dtype=gl.ANCHOR_DTYPE)
-    a["query"] = golden["query"] + golden["length"] // 2
-    a["target"] = golden["target"] + golden["length"] // 2
-    return seq, a, golden["query"] == golden["target"]
+    return seq, gl.ssp_anchors(golden), golden["query"] == golden["target"]
 
 
 def test_golden_sample_anchors_against_the_oracle(ce):
@@ -61,7 +59,7 @@ def test_golden_sample_anchors_against_the_oracle(ce):
 def test_synthetic_anchors_against_the_oracle(ce, n, divergence):
     from genomeworks_b200 import synth
     target, query, seeds = synth.extender_workload(5000, divergence, n, 0.3, seed=100 + n)
-    for matrix, o, e, y, threshold in ((xl.SAMPLE_MATRIX, *LASTZ, gl.LASTZ_THRESHOLD), (gl.SIMPLE_MATRIX, 5, 2, 80, 0)):
+    for matrix, o, e, y, threshold in ((xl.SAMPLE_MATRIX, *LASTZ, gl.LASTZ_THRESHOLD), (xl.SIMPLE_MATRIX, 5, 2, 80, 0)):
         want = gl.oracle_run(query, target, matrix, o, e, y, threshold, seeds)
         assert_equal(run_engine(ce, query, target, matrix, o, e, y, threshold, seeds), want)
 
@@ -73,10 +71,10 @@ def test_range_wider_than_the_shared_ring(ce):
     q = s.copy()
     q[rng.random(6000) < 0.1] = 4
     a = np.array([(0, 0), (3000, 3000), (5999, 5999)], dtype=gl.ANCHOR_DTYPE)
-    want = gl.oracle_run(q, s, gl.SIMPLE_MATRIX, 1, 0, 3000, -(1 << 40), a)
+    want = gl.oracle_run(q, s, xl.SIMPLE_MATRIX, 1, 0, 3000, -(1 << 40), a)
     # about 6000 x 6000 live cells per anchor: ranges of thousands of cells
     assert want[2] > 10 ** 7
-    assert_equal(run_engine(ce, q, s, gl.SIMPLE_MATRIX, 1, 0, 3000, -(1 << 40), a), want)
+    assert_equal(run_engine(ce, q, s, xl.SIMPLE_MATRIX, 1, 0, 3000, -(1 << 40), a), want)
 
 
 def test_side_of_about_one_megabase(ce):
@@ -99,13 +97,8 @@ def test_score_past_2_31(ce):
     assert_equal(got, want)
 
 
-def synthetic(n=300, seed=21):
-    from genomeworks_b200 import synth
-    return synth.extender_workload(30000, 0.15, n, 0.3, seed=seed)
-
-
 def test_many_rounds_equal_one_round(ce):
-    target, query, seeds = synthetic()
+    target, query, seeds = gl.synthetic()
     one = run_engine(ce, query, target, xl.SAMPLE_MATRIX, *LASTZ, gl.LASTZ_THRESHOLD, seeds)
     # the largest alignment's storage: every round holds one or two alignments
     sizes = [gl.oracle_side(query, target, xl.SAMPLE_MATRIX, *LASTZ, int(s["query"]), int(s["target"]), side, trace=False)["storage"]
@@ -134,7 +127,7 @@ def test_budget_below_one_alignment_gives_exact_intervals_without_cigar(ce):
 
 def test_device_pointer_api_equals_the_host_api(ce):
     import torch
-    target, query, seeds = synthetic(400, 23)
+    target, query, seeds = gl.synthetic(400, 23)
     ext = ce.create_extender(xl.SAMPLE_MATRIX, xl.SAMPLE_XDROP)
     dq = torch.from_numpy(query).cuda()
     dt = torch.from_numpy(target).cuda()
@@ -149,9 +142,7 @@ def test_device_pointer_api_equals_the_host_api(ce):
     g = ce.create_gapped_extender(xl.SAMPLE_MATRIX, *LASTZ)
     assert g.extend_ssps_device(dq, dt, gl.LASTZ_THRESHOLD, dout, n) == ce.success and g.sync() == ce.success
     got = g.get_alignments() + (g.last_live_cells(),)
-    a = np.zeros(n, dtype=gl.ANCHOR_DTYPE)
-    a["query"] = ssps[:, 0] + ssps[:, 2] // 2
-    a["target"] = ssps[:, 1] + ssps[:, 2] // 2
+    a = gl.ssp_anchors(np.ascontiguousarray(ssps).view(xl.SSP_DTYPE).reshape(-1))
     assert_equal(got, run_engine(ce, query, target, xl.SAMPLE_MATRIX, *LASTZ, gl.LASTZ_THRESHOLD, a))
     # an anchor outside the sequences is invalid_input at sync
     bad = dout[:1].clone()
@@ -163,7 +154,7 @@ def test_device_pointer_api_equals_the_host_api(ce):
 
 def test_reused_extender_equals_fresh_ones_and_a_stream(ce):
     import torch
-    cases = [synthetic(200, s) for s in (31, 32, 33)]
+    cases = [gl.synthetic(200, s) for s in (31, 32, 33)]
     ext = ce.create_gapped_extender(xl.SAMPLE_MATRIX, *LASTZ)
     stream = torch.cuda.Stream()
     on_stream = ce.create_gapped_extender(xl.SAMPLE_MATRIX, *LASTZ, stream=stream)
@@ -177,25 +168,8 @@ def test_reused_extender_equals_fresh_ones_and_a_stream(ce):
     on_stream.close()
 
 
-class CountingAllocator:
-    def __init__(self):
-        import torch
-        self.torch = torch
-        self.live = {}
-        self.calls = 0
-
-    def alloc(self, n):
-        t = self.torch.empty(int(n), dtype=self.torch.uint8, device="cuda")
-        self.live[t.data_ptr()] = t
-        self.calls += 1
-        return t.data_ptr()
-
-    def free(self, p, n):
-        del self.live[p]
-
-
 def test_allocator_balance(ce):
-    target, query, seeds = synthetic(200, 41)
+    target, query, seeds = gl.synthetic(200, 41)
     alloc = CountingAllocator()
     ext = ce.create_gapped_extender(xl.SAMPLE_MATRIX, *LASTZ, allocator=alloc)
     got = run_engine(ce, query, target, xl.SAMPLE_MATRIX, *LASTZ, gl.LASTZ_THRESHOLD, seeds, ext=ext)
@@ -207,7 +181,7 @@ def test_allocator_balance(ce):
 
 def test_cpp_program_agrees_with_python(ce, tmp_path):
     exe = os.path.join(ROOT, "build", "test_cpp_gapped_extender")
-    target, query, seeds = synthetic(150, 51)
+    target, query, seeds = gl.synthetic(150, 51)
     query.tofile(tmp_path / "q.bin")
     target.tofile(tmp_path / "t.bin")
     seeds.tofile(tmp_path / "a.bin")

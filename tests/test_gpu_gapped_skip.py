@@ -1,19 +1,17 @@
 """The skip-covered mode (DESIGN.md section 18) on the GPU against its CPU oracle: records, their order, CIGARs, has_cigar, live
 cells and the extended / skipped counts, for the gapped extender and the genome aligner; round sizes, budgets and block sizes
 do not change the output, and the mode does not leak into later default calls."""
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
 import extender_libs as xl
 import gapped_extender_libs as gl
 import gapped_skip_libs as sk
+import genome_aligner_libs as ga
 import seeder_libs as sl
+from checker_lib import CountingAllocator
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LASTZ = (xl.SAMPLE_MATRIX, gl.LASTZ_OPEN, gl.LASTZ_EXTEND, gl.LASTZ_YDROP)
 
 
@@ -44,8 +42,7 @@ def run_ssps(ce, seq_q, seq_t, params, threshold, ssps, budget=1 << 30, round_an
     import torch
     dq = torch.from_numpy(np.ascontiguousarray(seq_q, np.int8)).cuda()
     dt = torch.from_numpy(np.ascontiguousarray(seq_t, np.int8)).cuda()
-    ds = torch.from_numpy(np.stack([ssps["query"].astype(np.int64), ssps["target"].astype(np.int64), ssps["length"], ssps["score"]], 1)
-                          .astype(np.int32)).cuda()
+    ds = xl.ssps_on_device(ssps)
     x = ce.create_gapped_extender(*params, budget, skip_covered=True, round_anchors=round_anchors)
     assert x.extend_ssps_device(dq, dt, threshold, ds, len(ssps)) == ce.success
     out = finish(x, ce)
@@ -70,7 +67,7 @@ def golden():
 
 def test_golden_sample_ssps_on_the_device(ce):
     seq, ssps = golden()
-    want = sk.skip_run(seq, seq, *LASTZ, gl.LASTZ_THRESHOLD, sk.ssp_anchors(ssps), sk.ssp_order(ssps))
+    want = sk.skip_run(seq, seq, *LASTZ, gl.LASTZ_THRESHOLD, gl.ssp_anchors(ssps), sk.ssp_order(ssps))
     assert want[3]["skipped"] > 0
     got = run_ssps(ce, seq, seq, LASTZ, gl.LASTZ_THRESHOLD, ssps)
     assert_equal(got, want, len(ssps))
@@ -83,7 +80,7 @@ def test_host_anchors_in_the_ssp_order_equal_the_device_call(ce):
     seq, ssps = golden()
     order = sk.ssp_order(ssps)
     dev = run_ssps(ce, seq, seq, LASTZ, gl.LASTZ_THRESHOLD, ssps)
-    host = run_host(ce, seq, seq, LASTZ, gl.LASTZ_THRESHOLD, sk.ssp_anchors(ssps)[order])
+    host = run_host(ce, seq, seq, LASTZ, gl.LASTZ_THRESHOLD, gl.ssp_anchors(ssps)[order])
     rec = host[0].copy()
     rec["anchor"] = order[rec["anchor"]]
     assert gl.rows(rec) == gl.rows(dev[0]) and host[1:] == dev[1:]
@@ -94,7 +91,7 @@ def test_host_anchors_in_the_ssp_order_equal_the_device_call(ce):
 def test_synthetic_anchors_against_the_oracle(ce, n, divergence):
     from genomeworks_b200 import synth
     target, query, seeds = synth.extender_workload(5000, divergence, n, 0.3, seed=100 + n)
-    for params, threshold in ((LASTZ, gl.LASTZ_THRESHOLD), ((gl.SIMPLE_MATRIX, 5, 2, 80), 0)):
+    for params, threshold in ((LASTZ, gl.LASTZ_THRESHOLD), ((xl.SIMPLE_MATRIX, 5, 2, 80), 0)):
         want = sk.skip_run(query, target, *params, threshold, seeds)
         assert_equal(run_host(ce, query, target, params, threshold, seeds), want, n)
         if n == 1001:
@@ -108,20 +105,15 @@ def test_range_wider_than_the_shared_ring(ce):
     q = s.copy()
     q[rng.random(6000) < 0.1] = 4
     a = np.array([(3000, 3000), (0, 0), (5999, 5999), (1500, 1500)], dtype=gl.ANCHOR_DTYPE)
-    params = (gl.SIMPLE_MATRIX, 1, 0, 3000)
+    params = (xl.SIMPLE_MATRIX, 1, 0, 3000)
     want = sk.skip_run(q, s, *params, -(1 << 40), a)
     assert want[2] > 10 ** 7
     assert_equal(run_host(ce, q, s, params, -(1 << 40), a), want, len(a))
     assert_equal(run_host(ce, q, s, params, -(1 << 40), a, round_anchors=1), want, len(a))
 
 
-def synthetic(n=300, seed=21):
-    from genomeworks_b200 import synth
-    return synth.extender_workload(30000, 0.15, n, 0.3, seed=seed)
-
-
 def test_budgets_that_force_many_trace_rounds_or_no_cigar(ce):
-    target, query, seeds = synthetic()
+    target, query, seeds = gl.synthetic()
     full = sk.skip_run(query, target, *LASTZ, gl.LASTZ_THRESHOLD, seeds)
     sizes = [sum(gl.oracle_side(query, target, *LASTZ, int(seeds[k]["query"]), int(seeds[k]["target"]), side, trace=False)["storage"]
                  for side in (True, False)) for k in full[0]["anchor"]]
@@ -133,25 +125,8 @@ def test_budgets_that_force_many_trace_rounds_or_no_cigar(ce):
             assert_equal(run_host(ce, query, target, LASTZ, gl.LASTZ_THRESHOLD, seeds, budget, round_anchors=k), want, len(seeds))
 
 
-class CountingAllocator:
-    def __init__(self):
-        import torch
-        self.torch = torch
-        self.live = {}
-        self.calls = 0
-
-    def alloc(self, n):
-        t = self.torch.empty(int(n), dtype=self.torch.uint8, device="cuda")
-        self.live[t.data_ptr()] = t
-        self.calls += 1
-        return t.data_ptr()
-
-    def free(self, p, n):
-        del self.live[p]
-
-
 def test_mode_does_not_leak_and_allocator_balances(ce):
-    target, query, seeds = synthetic(400, 41)
+    target, query, seeds = gl.synthetic(400, 41)
     default = gl.oracle_run(query, target, *LASTZ, gl.LASTZ_THRESHOLD, seeds)
     alloc = CountingAllocator()
     x = ce.create_gapped_extender(*LASTZ, allocator=alloc, skip_covered=True, round_anchors=5)
@@ -170,33 +145,9 @@ def test_mode_does_not_leak_and_allocator_balances(ce):
     assert alloc.live == {}
 
 
-def check_aligner(ce, targets, queries, strand="both", **params):
-    al = ce.GenomeAligner(strand, skip_covered=True, **params)
-    rec, cigars = al.run(targets, queries)
-    stats = al.last_skip_stats()
-    al.close()
-    rows, want_cigars, want_stats = sk.aligner_skip_oracle(targets, queries, strand,
-                                                           **{k: v for k, v in params.items() if k not in ("block_size", "round_anchors")})
-    assert sl.engine_rows(rec) == rows
-    assert cigars == want_cigars
-    assert (stats["extended"], stats["skipped"]) == (want_stats["extended"], want_stats["skipped"])
-    return rec, cigars, stats
-
-
-def records_case():
-    rng = np.random.default_rng(17)
-    shared = rng.integers(0, 4, 6000).astype(np.int8)
-    targets = [np.concatenate([rng.integers(0, 4, 2000).astype(np.int8), shared[:3000]]),
-               rng.integers(0, 4, 4000).astype(np.int8),
-               np.concatenate([sl.reverse_complement(shared[2500:]), rng.integers(0, 4, 1000).astype(np.int8)])]
-    queries = [sl.mutate(shared, 0.03, rng), np.concatenate([rng.integers(0, 4, 500).astype(np.int8), sl.mutate(targets[1][1000:3000], 0.05, rng)])]
-    queries[1][100:140] = 5
-    return targets, queries
-
-
 def test_aligner_golden_sample_both_strands(ce):
     seq, _ = golden()
-    rec, _, stats = check_aligner(ce, [seq], [seq])
+    rec, _, stats, _ = ga.check_aligner(ce, [seq], [seq], skip=True)
     assert (rec["strand"] == 1).any() and stats["skipped"] > 0
     default, _ = ce.align_genomes([seq], [seq])
     assert len(rec) <= len(default)
@@ -204,29 +155,21 @@ def test_aligner_golden_sample_both_strands(ce):
 
 def test_aligner_inversion_pair_and_records(ce):
     target, query, _ = sl.rearranged_pair(5)
-    rec, _, _ = check_aligner(ce, [target], [query])
+    rec, _, _, _ = ga.check_aligner(ce, [target], [query], skip=True)
     assert (rec["strand"] == 1).any()
-    targets, queries = records_case()
-    want = check_aligner(ce, targets, queries)
+    targets, queries = ga.records_case()
+    want = ga.check_aligner(ce, targets, queries, skip=True)
     # blocks of 7 seeds and rounds of 7 anchors give the same output
-    got = check_aligner(ce, targets, queries, block_size=7, round_anchors=7)
-    assert sl.engine_rows(got[0]) == sl.engine_rows(want[0]) and got[1] == want[1]
+    got = ga.check_aligner(ce, targets, queries, skip=True, block_size=7, round_anchors=7)
+    assert ga.engine_rows(got[0]) == ga.engine_rows(want[0]) and got[1] == want[1]
     # the rule's counts do not depend on the rounds; speculative and rounds describe the grouping itself
     assert all(got[2][k] == want[2][k] for k in ("extended", "skipped", "traced"))
 
 
 def test_tool_skip_covered_prints_the_same_paf(ce, tmp_path):
-    targets, queries = records_case()
-    tnames, qnames = ["t%d" % k for k in range(3)], ["q%d" % k for k in range(2)]
-    with open(tmp_path / "t.fa", "w") as f:
-        for n, s in zip(tnames, targets):
-            f.write(">%s\n%s\n" % (n, sl.text(s)))
-    with open(tmp_path / "q.fa", "w") as f:
-        for n, s in zip(qnames, queries):
-            f.write(">%s\n%s\n" % (n, sl.text(s)))
+    targets, queries = ga.records_case()
     rec, cigars = ce.align_genomes(targets, queries, skip_covered=True)
-    want = ce.format_paf(rec, cigars, tnames, [len(s) for s in targets], qnames, [len(s) for s in queries])
-    out = subprocess.run([os.path.join(ROOT, "build", "cudaextender"), "--skip-covered", str(tmp_path / "t.fa"), str(tmp_path / "q.fa")],
-                         capture_output=True, text=True, timeout=600)
+    want = ga.tool_paf(ce, rec, cigars, targets, queries)
+    out = ga.run_tool(tmp_path, targets, queries, "--skip-covered")
     assert out.returncode == 0, out.stderr
     assert out.stdout == want and want

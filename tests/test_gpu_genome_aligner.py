@@ -2,18 +2,14 @@
 complement and coordinate mapping, the PAF rules in Python): records, CIGARs and PAF, on the golden sample, a rearranged pair
 and several records per side; every CIGAR re-scores to its score, the block size does not change the output, and the
 cudaextender tool prints the same PAF."""
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
 import extender_libs as xl
-import gapped_extender_libs as gl
+import genome_aligner_libs as ga
 import seeder_libs as sl
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -24,36 +20,15 @@ def ce():
     return cudaextender
 
 
-def check_against_oracle(ce, targets, queries, strand="both", **params):
-    rec, cigars = ce.align_genomes(targets, queries, strand=strand, **params)
-    rows, want_cigars, anchors = sl.aligner_oracle(targets, queries, strand, **params)
-    assert sl.engine_rows(rec) == rows
-    assert cigars == want_cigars
-    # every CIGAR re-scores to its score, on its strand's query
-    for r, cg, (q0, t0) in zip(rec, cigars, anchors):
-        if not r["has_cigar"]:
-            continue
-        q = np.asarray(queries[r["query_record"]], np.int8)
-        qs = sl.reverse_complement(q) if r["strand"] else q
-        qb = len(q) - int(r["query_end"]) if r["strand"] else int(r["query_begin"])
-        score, qn, tn = gl.rescore(cg, qs, targets[r["target_record"]], sl.DEFAULTS["matrix"], gl.LASTZ_OPEN, gl.LASTZ_EXTEND, qb,
-                                   int(r["target_begin"]), anchor=(q0, t0))
-        assert (score, qn, tn) == (int(r["score"]), int(r["query_end"] - r["query_begin"]), int(r["target_end"] - r["target_begin"]))
-    return rec, cigars
-
-
 def test_golden_sample_both_strands(ce):
     seq, _, _ = xl.sample()
-    rec, cigars = check_against_oracle(ce, [seq], [seq])
+    rec = ga.check_aligner(ce, [seq], [seq])[0]
     assert (rec["strand"] == 0).sum() > 0
-    names, lengths = ["sample"], [len(seq)]
-    assert ce.format_paf(rec, cigars, names, lengths, names, lengths) == sl.paf_oracle(sl.engine_rows(rec), cigars, names, lengths, names,
-                                                                                        lengths)
 
 
 def test_rearranged_pair_finds_the_inversion_on_the_minus_strand(ce):
     target, query, (a, b) = sl.rearranged_pair(5)
-    rec, _ = check_against_oracle(ce, [target], [query])
+    rec = ga.check_aligner(ce, [target], [query])[0]
     minus = rec[rec["strand"] == 1]
     # the inverted piece sits at about [a, b) in both: a minus-strand alignment covers most of it at forward coordinates
     hit = [r for r in minus if r["target_begin"] < b and r["target_end"] > a and abs(int(r["query_begin"]) - int(r["target_begin"])) < 500
@@ -64,20 +39,9 @@ def test_rearranged_pair_finds_the_inversion_on_the_minus_strand(ce):
     assert (np.abs(plus["query_begin"].astype(np.int64) - plus["target_begin"].astype(np.int64)) > 2000).any()
 
 
-def records_case():
-    rng = np.random.default_rng(17)
-    shared = rng.integers(0, 4, 6000).astype(np.int8)
-    targets = [np.concatenate([rng.integers(0, 4, 2000).astype(np.int8), shared[:3000]]),
-               rng.integers(0, 4, 4000).astype(np.int8),
-               np.concatenate([sl.reverse_complement(shared[2500:]), rng.integers(0, 4, 1000).astype(np.int8)])]
-    queries = [sl.mutate(shared, 0.03, rng), np.concatenate([rng.integers(0, 4, 500).astype(np.int8), sl.mutate(targets[1][1000:3000], 0.05, rng)])]
-    queries[1][100:140] = 5
-    return targets, queries
-
-
 def test_three_targets_by_two_queries(ce):
-    targets, queries = records_case()
-    rec, _ = check_against_oracle(ce, targets, queries)
+    targets, queries = ga.records_case()
+    rec = ga.check_aligner(ce, targets, queries)[0]
     assert set(zip(rec["target_record"].tolist(), rec["query_record"].tolist())) >= {(0, 0), (2, 0), (1, 1)}
     order = [(int(r["target_record"]), int(r["query_record"]), int(r["strand"])) for r in rec]
     assert order == sorted(order)
@@ -85,54 +49,44 @@ def test_three_targets_by_two_queries(ce):
 
 def test_block_size_does_not_change_the_output(ce):
     seq, _, _ = xl.sample()
-    targets, queries = records_case()
+    targets, queries = ga.records_case()
     for t, q in (([seq], [seq]), (targets, queries)):
         want = ce.align_genomes(t, q)
         for b in (1000, 7):
             if b == 7 and len(t) == 1:
                 continue  # 143,671 seeds in blocks of 7 is slow, not different
             got = ce.align_genomes(t, q, block_size=b)
-            assert sl.engine_rows(got[0]) == sl.engine_rows(want[0]) and got[1] == want[1]
+            assert ga.engine_rows(got[0]) == ga.engine_rows(want[0]) and got[1] == want[1]
 
 
 def test_one_strand_and_exact_seeds(ce):
-    targets, queries = records_case()
+    targets, queries = ga.records_case()
     for strand in ("plus", "minus"):
-        check_against_oracle(ce, targets, queries, strand=strand)
-    check_against_oracle(ce, targets[:1], queries[:1], transition=False)
+        ga.check_aligner(ce, targets, queries, strand=strand)
+    ga.check_aligner(ce, targets[:1], queries[:1], transition=False)
 
 
 def test_tool_prints_the_same_paf(ce, tmp_path):
-    targets, queries = records_case()
-    tnames, qnames = ["t%d extra words" % k for k in range(3)], ["q%d" % k for k in range(2)]
-    with open(tmp_path / "t.fa", "w") as f:
-        for n, s in zip(tnames, targets):
-            f.write(">%s\n%s\n" % (n, sl.text(s)))
-    with open(tmp_path / "q.fq", "w") as f:
-        for n, s in zip(qnames, queries):
-            f.write("@%s\n%s\n+\n%s\n" % (n, sl.text(s), "I" * len(s)))
+    targets, queries = ga.records_case()
     rec, cigars = ce.align_genomes(targets, queries)
-    want = ce.format_paf(rec, cigars, [n.split()[0] for n in tnames], [len(s) for s in targets], qnames, [len(s) for s in queries])
-    assert want == sl.paf_oracle(sl.engine_rows(rec), cigars, [n.split()[0] for n in tnames], [len(s) for s in targets], qnames,
-                                 [len(s) for s in queries])
-    out = subprocess.run([os.path.join(ROOT, "build", "cudaextender"), str(tmp_path / "t.fa"), str(tmp_path / "q.fq")], capture_output=True,
-                         text=True, timeout=600)
+    want = ga.tool_paf(ce, rec, cigars, targets, queries)
+    assert want == ga.paf_oracle(ga.engine_rows(rec), cigars, ga.names("t", targets), ga.lengths(targets), ga.names("q", queries),
+                                 ga.lengths(queries))
+    out = ga.run_tool(tmp_path, targets, queries, fastq=True)
     assert out.returncode == 0, out.stderr
     assert out.stdout == want and want
-    out = subprocess.run([os.path.join(ROOT, "build", "cudaextender"), "-s", "minus", "-B", "1000", str(tmp_path / "t.fa"), str(tmp_path / "q.fq")],
-                         capture_output=True, text=True, timeout=600)
+    out = ga.run_tool(tmp_path, targets, queries, "-s", "minus", "-B", "1000", fastq=True)
     rec, cigars = ce.align_genomes(targets, queries, strand="minus")
-    assert out.returncode == 0 and out.stdout == ce.format_paf(rec, cigars, [n.split()[0] for n in tnames], [len(s) for s in targets], qnames,
-                                                               [len(s) for s in queries])
+    assert out.returncode == 0 and out.stdout == ga.tool_paf(ce, rec, cigars, targets, queries)
 
 
 def test_stats_and_a_stream(ce):
     import torch
-    targets, queries = records_case()
+    targets, queries = ga.records_case()
     want = ce.align_genomes(targets, queries)
     al = ce.GenomeAligner(stream=torch.cuda.Stream())
     got = al.run(targets, queries)
-    assert sl.engine_rows(got[0]) == sl.engine_rows(want[0]) and got[1] == want[1]
+    assert ga.engine_rows(got[0]) == ga.engine_rows(want[0]) and got[1] == want[1]
     ms, counts = al.last_stats()
     assert ms["index"] > 0 and ms["count"] > 0 and ms["write"] > 0 and ms["ungapped"] > 0 and ms["gapped_pass1"] > 0
     assert counts["seeds"] > counts["ssps"] > 0 and counts["alignments"] == len(got[0])

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import index_libs as il
+from checker_lib import CountingAllocator
 
 pytestmark = pytest.mark.gpu
 
@@ -127,26 +128,6 @@ def test_launch_count_independent_of_read_count(cm):
         counts.append(lib().gwb200_kernel_launch_count() - before)
         idx.close()
     assert counts[0] == counts[1] == counts[2] > 0, counts
-
-
-class CountingAllocator:
-    """Device memory from torch's caching allocator; counts what is outstanding."""
-
-    def __init__(self):
-        import torch
-        self.torch = torch
-        self.live = {}
-        self.calls = 0
-
-    def alloc(self, n):
-        p = self.torch.cuda.caching_allocator_alloc(int(n))
-        self.live[p] = n
-        self.calls += 1
-        return p
-
-    def free(self, p, n):
-        assert self.live.pop(p) == n
-        self.torch.cuda.caching_allocator_delete(p)
 
 
 def test_all_device_memory_returns_to_the_allocator(cm):

@@ -9,6 +9,7 @@ import pytest
 
 import index_libs as il
 import matcher_libs as ml
+from checker_lib import CountingAllocator
 
 pytestmark = pytest.mark.gpu
 
@@ -183,29 +184,6 @@ def test_widest_key_against_oracle(cm):
     got, bits = run(cm, qd.arrays, td.arrays)
     assert bits == ml.key_bits(top - 5, top - 1, top - 7, top - 1) > 120
     same(got, ml.oracle_run(qs, ts))
-
-
-class CountingAllocator:
-    """Device memory from torch's caching allocator; counts what is outstanding, and can refuse its n-th request."""
-
-    def __init__(self, refuse=None):
-        import torch
-        self.torch = torch
-        self.live = {}
-        self.calls = 0
-        self.refuse = refuse
-
-    def alloc(self, n):
-        self.calls += 1
-        if self.calls == self.refuse:
-            return 0
-        p = self.torch.cuda.caching_allocator_alloc(int(n))
-        self.live[p] = n
-        return p
-
-    def free(self, p, n):
-        assert self.live.pop(p) == n
-        self.torch.cuda.caching_allocator_delete(p)
 
 
 def test_more_than_int_max_anchors_rejected_before_allocating_them(cm):

@@ -10,6 +10,7 @@ import pytest
 import index_libs as il
 import matcher_libs as ml
 import overlapper_libs as ol
+from checker_lib import CountingAllocator
 
 pytestmark = pytest.mark.gpu
 
@@ -169,29 +170,6 @@ def test_launch_count_independent_of_anchor_count(cm):
     assert counts[:4] == [counts[0]] * 4 and counts[0] > 0 and counts[4] == 0, counts
     assert ov.last_kernel_ms() == -1.0  # nothing ran for n == 0
     ov.close()
-
-
-class CountingAllocator:
-    """Device memory from torch's caching allocator; counts what is outstanding, and can refuse its n-th request."""
-
-    def __init__(self, refuse=None):
-        import torch
-        self.torch = torch
-        self.live = {}
-        self.calls = 0
-        self.refuse = refuse
-
-    def alloc(self, n):
-        self.calls += 1
-        if self.calls == self.refuse:
-            return 0
-        p = self.torch.cuda.caching_allocator_alloc(int(n))
-        self.live[p] = n
-        return p
-
-    def free(self, p, n):
-        assert self.live.pop(p) == n
-        self.torch.cuda.caching_allocator_delete(p)
 
 
 def test_allocator_balance_and_refusal(cm):

@@ -10,6 +10,7 @@ import pytest
 
 import index_libs as il
 import rescue_libs as rl
+from checker_lib import CountingAllocator
 
 pytestmark = pytest.mark.gpu
 
@@ -99,29 +100,6 @@ def test_pipeline_index_matcher_overlapper_rescue_against_oracle_chain(cm):
     assert rl.ol.rows(res) != rl.ol.rows(got)
     for x in (ov, m, idx):
         x.close()
-
-
-class CountingAllocator:
-    """Device memory from torch's caching allocator; counts what is outstanding, and can refuse its n-th request."""
-
-    def __init__(self, refuse=None):
-        import torch
-        self.torch = torch
-        self.live = {}
-        self.calls = 0
-        self.refuse = refuse
-
-    def alloc(self, n):
-        self.calls += 1
-        if self.calls == self.refuse:
-            return 0
-        p = self.torch.cuda.caching_allocator_alloc(int(n))
-        self.live[p] = n
-        return p
-
-    def free(self, p, n):
-        assert self.live.pop(p) == n
-        self.torch.cuda.caching_allocator_delete(p)
 
 
 def test_rejections_leave_the_overlaps_unchanged(cm):

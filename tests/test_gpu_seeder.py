@@ -5,6 +5,7 @@ import pytest
 
 import extender_libs as xl
 import seeder_libs as sl
+from checker_lib import CountingAllocator
 
 pytestmark = pytest.mark.gpu
 
@@ -26,7 +27,7 @@ def blocks(seeder, n, size):
     """Seeds [0, n) fetched in blocks of `size`, concatenated."""
     parts = [seeder.get_block(first, min(size, n - first)) for first in range(0, n, size)]
     seeder.sync()
-    out = np.zeros(n, dtype=sl.SEED_DTYPE)
+    out = np.zeros(n, dtype=xl.SEED_DTYPE)
     if n:
         h = np.concatenate([p.cpu().numpy() for p in parts])
         out["query"], out["target"] = h[:, 0].view(np.uint32), h[:, 1].view(np.uint32)
@@ -115,7 +116,7 @@ def blocks_from(seeder, first, count):
     d = seeder.get_block(first, count)
     seeder.sync()
     h = d.cpu().numpy()
-    out = np.zeros(count, dtype=sl.SEED_DTYPE)
+    out = np.zeros(count, dtype=xl.SEED_DTYPE)
     out["query"], out["target"] = h[:, 0].view(np.uint32), h[:, 1].view(np.uint32)
     return out
 
@@ -137,23 +138,6 @@ def test_device_sequences(ce):
     n = s.count(torch.from_numpy(query).cuda())
     assert_same(blocks(s, n, n), sl.oracle_run(query, target, True))
     s.close()
-
-
-class CountingAllocator:
-    def __init__(self):
-        import torch
-        self.torch = torch
-        self.live = {}
-        self.calls = 0
-
-    def alloc(self, n):
-        t = self.torch.empty(int(n), dtype=self.torch.uint8, device="cuda")
-        self.live[t.data_ptr()] = t
-        self.calls += 1
-        return t.data_ptr()
-
-    def free(self, p, n):
-        del self.live[p]
 
 
 def test_reused_across_targets_with_a_stream_and_an_allocator(ce):

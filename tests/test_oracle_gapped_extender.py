@@ -4,10 +4,10 @@ import numpy as np
 import pytest
 
 import gapped_extender_libs as gl
-from extender_libs import SAMPLE_MATRIX as SAMPLE
+from extender_libs import SAMPLE_MATRIX as SAMPLE, SIMPLE_MATRIX
 from genomeworks_b200.cudaextender import encode_sequence
 
-M10 = gl.SIMPLE_MATRIX  # +10 / -10 among A/C/G/T
+M10 = SIMPLE_MATRIX  # +10 / -10 among A/C/G/T
 
 
 def anchors(*pairs):
@@ -143,7 +143,7 @@ def test_every_cigar_consumes_its_intervals_and_rescores_to_its_score(divergence
     from genomeworks_b200 import synth
     target, query, seeds = synth.extender_workload(3000, divergence, 60, 0.3, seed=5)
     for o, e, y in ((400, 30, 9400), (5, 2, 60), (0, 1, 30)):
-        mat = gl.SIMPLE_MATRIX if o < 100 else SAMPLE
+        mat = SIMPLE_MATRIX if o < 100 else SAMPLE
         rec, cig, _ = gl.oracle_run(query, target, mat, o, e, y, -(1 << 40), seeds)
         assert len(rec) > 0
         for r, c in zip(rec, cig):

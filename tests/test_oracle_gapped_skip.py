@@ -7,7 +7,7 @@ import extender_libs as xl
 import gapped_extender_libs as gl
 import gapped_skip_libs as sk
 
-SIMPLE = (gl.SIMPLE_MATRIX, 5, 2, 80)
+SIMPLE = (xl.SIMPLE_MATRIX, 5, 2, 80)
 LASTZ = (xl.SAMPLE_MATRIX, gl.LASTZ_OPEN, gl.LASTZ_EXTEND, gl.LASTZ_YDROP)
 
 
@@ -90,7 +90,7 @@ def test_ssp_score_ties_go_to_the_smaller_index():
     ssps["score"] = [7, 9, 9, 7]
     order = sk.ssp_order(ssps)
     assert order.tolist() == [1, 2, 0, 3]
-    (rec, _, _, stats), skipped = both(s, s, SIMPLE, 0, sk.ssp_anchors(ssps), order)
+    (rec, _, _, stats), skipped = both(s, s, SIMPLE, 0, gl.ssp_anchors(ssps), order)
     assert [int(r["anchor"]) for r in rec] == [1] and skipped == [2, 0, 3]
 
 
@@ -118,13 +118,13 @@ def test_random_cases(seed):
     o, e, y = int(rng.integers(0, 12)), int(rng.integers(0, 5)), int(rng.integers(10, 120))
     threshold = int(rng.integers(-50, 200))
     budget = [1 << 62, int(rng.integers(0, 3000)), 0][int(rng.integers(0, 3))]
-    both(q, t, (gl.SIMPLE_MATRIX, o, e, y), threshold, a, order, budget)
+    both(q, t, (xl.SIMPLE_MATRIX, o, e, y), threshold, a, order, budget)
 
 
 def test_golden_sample_subset_and_coverage_against_the_default_oracle():
     seq, _, golden = xl.sample()
     assert len(golden) == 1337
-    a = sk.ssp_anchors(golden)
+    a = gl.ssp_anchors(golden)
     order = sk.ssp_order(golden)
     rec, cig, live, stats = sk.skip_run(seq, seq, *LASTZ, gl.LASTZ_THRESHOLD, a, order)
     full_rec, full_cig, full_live = gl.oracle_run(seq, seq, *LASTZ, gl.LASTZ_THRESHOLD, a)
