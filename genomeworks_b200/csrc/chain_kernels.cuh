@@ -198,5 +198,111 @@ __global__ void __launch_bounds__(1024) chain_finish_kernel(const int64_t* __res
     res[1] = bv;
 }
 
+// ---- every chain above a minimum score (DESIGN.md section 20), on top of the f and p above ----
+
+constexpr int kClaimThreads      = 1024;
+constexpr int32_t kClaimStagedMax = 28 * 1024; // SSPs whose p and owner marks (8 bytes each, 224 KiB) fit in shared memory
+
+// The priority order is f descending, ties to the smallest index: an ascending key ~(f with its sign bit flipped), sorted stably
+// with idx[k] = k.
+__global__ void chain_priority_keys_kernel(const int64_t* __restrict__ f, int32_t n, uint64_t* __restrict__ keys, int32_t* __restrict__ idx)
+{
+    for (int32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x)
+    {
+        keys[k] = ~(uint64_t(f[k]) ^ (uint64_t(1) << 63));
+        idx[k]  = k;
+    }
+}
+
+// One CTA: the claim walk. order[r] is the SSP of priority rank r. Every unclaimed SSP h, in priority order, heads chain c (the
+// next ordinal): h, p(h), p(p(h)), ... are claimed (owner = c) up to -1 or the first SSP already claimed. With `staged`, p and the
+// owner marks live in 8n bytes of dynamic shared memory; otherwise in global memory. Warp 0 reads the next 32 ranks and their
+// marks at once; a mark seen as claimed stays claimed, so only the open ones are re-read by the walking lane.
+__global__ void __launch_bounds__(kClaimThreads) chain_claim_kernel(const int32_t* __restrict__ order, const int32_t* p_g, int32_t n, int32_t staged,
+                                                                    int32_t* owner_g, int32_t* __restrict__ heads, int32_t* __restrict__ count)
+{
+    extern __shared__ int32_t smem[];
+    __shared__ int32_t batch[32];
+    const int32_t* p = p_g;
+    int32_t* owner   = owner_g;
+    if (staged)
+    {
+        p     = smem;
+        owner = smem + n;
+        for (int32_t x = threadIdx.x; x < n; x += blockDim.x)
+            smem[x] = p_g[x];
+    }
+    for (int32_t x = threadIdx.x; x < n; x += blockDim.x)
+        owner[x] = -1;
+    __syncthreads();
+    if (threadIdx.x < 32)
+    {
+        const int lane = threadIdx.x;
+        int32_t c      = 0;
+        for (int32_t r0 = 0; r0 < n; r0 += 32)
+        {
+            const int32_t h    = r0 + lane < n ? order[r0 + lane] : -1;
+            unsigned open      = __ballot_sync(0xffffffffu, h >= 0 && owner[h] < 0);
+            batch[lane]        = h;
+            __syncwarp();
+            if (lane == 0)
+                while (open)
+                {
+                    int32_t k = batch[__ffs(open) - 1];
+                    open &= open - 1;
+                    if (owner[k] >= 0)
+                        continue;
+                    heads[c] = k;
+                    for (; k >= 0 && owner[k] < 0; k = p[k])
+                        owner[k] = c;
+                    ++c;
+                }
+            __syncwarp();
+        }
+        if (lane == 0)
+            *count = c;
+    }
+    __syncthreads();
+    if (staged)
+        for (int32_t x = threadIdx.x; x < n; x += blockDim.x)
+            owner_g[x] = owner[x];
+}
+
+// One thread per SSP. k is the first member of its chain c when p(k) = -1 or p(k) belongs to another chain; exactly one member
+// is, and it writes the chain's score f(head) - f(k) + s(k). len[c] counts the members (zeroed before).
+__global__ void chain_score_kernel(const SspD* __restrict__ ssps, const int64_t* __restrict__ f, const int32_t* __restrict__ p,
+                                   const int32_t* __restrict__ owner, const int32_t* __restrict__ heads, int32_t n, int64_t* __restrict__ score,
+                                   int32_t* __restrict__ len)
+{
+    for (int32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x)
+    {
+        const int32_t c = owner[k], pk = p[k];
+        atomicAdd(&len[c], 1);
+        if (pk < 0 || owner[pk] != c)
+            score[c] = f[heads[c]] - f[k] + ssps[k].score;
+    }
+}
+
+// One thread per SSP and per chain. member[k]: k's chain is kept (score >= S); skey[k] = its chain for a member, n otherwise, and
+// sval[k] = k, for the stable sort into (chain, index). keep[c] for c < *count (zero beyond), and the kept scores summed into *sum.
+__global__ void chain_keep_kernel(const int32_t* __restrict__ owner, const int64_t* __restrict__ score, const int32_t* __restrict__ count, int32_t n,
+                                  int64_t S, uint8_t* __restrict__ member, uint8_t* __restrict__ keep, uint32_t* __restrict__ skey,
+                                  int32_t* __restrict__ sval, unsigned long long* __restrict__ sum)
+{
+    const int32_t chains = *count;
+    for (int32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x)
+    {
+        const int32_t c = owner[k];
+        const bool m    = score[c] >= S;
+        member[k]       = m;
+        skey[k]         = uint32_t(m ? c : n);
+        sval[k]         = k;
+        const bool kc   = k < chains && score[k] >= S;
+        keep[k]         = kc;
+        if (kc)
+            atomicAdd(sum, static_cast<unsigned long long>(score[k])); // mod 2^64: the int64 sum in any order
+    }
+}
+
 } // namespace chain
 } // namespace gwb200

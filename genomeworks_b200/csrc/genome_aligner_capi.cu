@@ -8,7 +8,8 @@
 // device; their alignments come back with CIGARs, and the host maps minus-strand query intervals to forward coordinates and
 // counts the PAF columns. In skip-covered mode (DESIGN.md section 18) the gapped extender of each pair and strand runs the
 // sequential rule in its own coordinates. With chaining on (DESIGN.md section 19) the unique segments of each pair and strand
-// are chained first, and only the chain's segments go to the gapped extender.
+// are chained first, and only the chain's segments go to the gapped extender; with all chains on (DESIGN.md section 20), the
+// union of every chain scoring at least the minimum does.
 
 #include "../../include/gwb200.h"
 #include "chain_internal.cuh"
@@ -80,6 +81,8 @@ struct gwb200_genome_aligner
     gwb200_ssp_chainer* chainer    = nullptr;
     bool chain_on        = false;
     int32_t chain_pen[2] = {0, 0}; // diagonal, anti-diagonal
+    bool chain_all       = false;  // every chain scoring >= chain_min instead of the best one
+    int64_t chain_min    = 0;
 
     DevBuf<int8_t> target_d{&hooks}, query_d{&hooks}, rc_d{&hooks};
     const int8_t* target_h = nullptr; // the host codes of the indexed target record
@@ -98,6 +101,7 @@ struct gwb200_genome_aligner
     int64_t n_seeds = 0, n_ssps = 0;
     int64_t skip_stats[5] = {}; // the gapped extender's, summed over pairs and strands
     gwb200_chain_stats chain_stats{};
+    int64_t chain_count = 0;
 
     ~gwb200_genome_aligner()
     {
@@ -223,12 +227,18 @@ int align_pair(gwb200_genome_aligner* a, int32_t ti, int32_t qi, int32_t strand,
     {
         if (!a->chained_d.ensure(n_ssps))
             return bad_alloc();
-        if (const int rc = chain::chain_ssps(a->chainer, a->ssps_d.p, n_ssps, a->chain_pen[0], a->chain_pen[1], a->chained_d.p))
+        if (const int rc = a->chain_all ? chain::chain_all_ssps(a->chainer, a->ssps_d.p, n_ssps, a->chain_pen[0], a->chain_pen[1], a->chain_min,
+                                                                a->chained_d.p)
+                                        : chain::chain_ssps(a->chainer, a->ssps_d.p, n_ssps, a->chain_pen[0], a->chain_pen[1], a->chained_d.p))
             return rc;
-        n_anchors = gwb200_ssp_chainer_num_chained(a->chainer);
-        float ms  = -1.f;
+        n_anchors            = gwb200_ssp_chainer_num_chained(a->chainer);
+        const int32_t chains = gwb200_ssp_chainer_num_chains(a->chainer);
+        float ms             = -1.f;
         if (n_anchors < 0)
             return n_anchors;
+        if (chains < 0)
+            return chains;
+        a->chain_count += chains;
         if (const int rc = gwb200_ssp_chainer_last_ms(a->chainer, &ms))
             return rc;
         anchors = a->chained_d.p;
@@ -333,6 +343,7 @@ void clear(gwb200_genome_aligner* a)
     a->n_seeds = a->n_ssps = 0;
     std::fill(a->skip_stats, a->skip_stats + 5, int64_t(0));
     a->chain_stats = gwb200_chain_stats{};
+    a->chain_count = 0;
 }
 
 int run(gwb200_genome_aligner* a, const int8_t* targets, const int64_t* toff, int32_t nt, const int8_t* queries, const int64_t* qoff, int32_t nq)
@@ -563,6 +574,25 @@ int gwb200_genome_aligner_last_chain_stats(const gwb200_genome_aligner* a, gwb20
     if (!a->ready)
         return set_error(GWB200_E_RUNTIME, "no finished run: call gwb200_genome_aligner_run first");
     *out = a->chain_stats;
+    return 0;
+}
+
+int gwb200_genome_aligner_set_chain_min_score(gwb200_genome_aligner* a, int32_t on, int64_t min_score)
+{
+    if (!a)
+        return set_error(GWB200_E_INVALID_ARGUMENT, "null genome aligner");
+    a->chain_all = on != 0;
+    a->chain_min = min_score;
+    return GWB200_EXT_SUCCESS;
+}
+
+int gwb200_genome_aligner_last_chain_count(const gwb200_genome_aligner* a, int64_t* chains)
+{
+    if (!a || !chains)
+        return set_error(GWB200_E_INVALID_ARGUMENT, "null argument");
+    if (!a->ready)
+        return set_error(GWB200_E_RUNTIME, "no finished run: call gwb200_genome_aligner_run first");
+    *chains = a->chain_count;
     return 0;
 }
 

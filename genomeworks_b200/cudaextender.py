@@ -8,8 +8,9 @@
 Sequences are int8 arrays of codes or str (encoded with encode_sequence); seed pairs are a structured array with named
 `query` and `target` fields (SEED_DTYPE), so the CSV's target-first column order cannot be confused with the record order.
 create_gapped_extender (GappedXDrop) turns anchors into gapped alignments with CIGARs. create_seeder (Seeder) makes the seed
-pairs of two sequences, create_ssp_chainer (SspChainer) finds the highest-scoring colinear chain of scored segment pairs,
-and align_genomes / format_paf run seeding, both extension stages and, optionally, chaining over two sets of records.
+pairs of two sequences, create_ssp_chainer (SspChainer) finds the highest-scoring colinear chain of scored segment pairs, or
+every chain above a minimum score, and align_genomes / format_paf run seeding, both extension stages and, optionally, chaining
+over two sets of records.
 There is no CPU fallback: without a CUDA device create_extender and create_gapped_extender raise.
 """
 import ctypes as C
@@ -369,6 +370,7 @@ def create_seeder(transition=True, stream=None, device_id=0, allocator=None):
 # Chaining (DESIGN.md section 19): the highest-scoring colinear chain of scored segment pairs.
 MAX_CHAIN_PENALTY = 1 << 20
 CHAIN_STATS = ("ssps_in", "ssps_chained", "pairs", "chain_ms")
+INT64_MIN, INT64_MAX = -(1 << 63), (1 << 63) - 1
 
 
 def _penalty(name, v):
@@ -390,9 +392,30 @@ def _chain_arg(chain):
     raise TypeError("chain must be None, True or a (diag_penalty, anti_penalty) pair")
 
 
+def _min_score(name, v):
+    """A minimum chain score (DESIGN.md section 20): any int64, checked before any device work."""
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+        raise TypeError("%s must be an integer" % name)
+    if not INT64_MIN <= int(v) <= INT64_MAX:
+        raise ValueError("%s must lie in [-2^63, 2^63 - 1]" % name)
+    return int(v)
+
+
+def _chain_args(chain, min_chain_score):
+    """(penalties or None, minimum chain score or None) of the aligner's chain arguments, checked before any device work."""
+    penalties = _chain_arg(chain)
+    if min_chain_score is None:
+        return penalties, None
+    min_score = _min_score("min_chain_score", min_chain_score)
+    if penalties is None:
+        raise ValueError("min_chain_score needs chain=True or (diag_penalty, anti_penalty)")
+    return penalties, min_score
+
+
 class SspChainer:
     """The chaining DP of DESIGN.md section 19 on the device: chain(ssps) returns the SSP indices of the highest-scoring colinear
-    chain, in ascending order, and its score; get_dp() returns f and p of every SSP."""
+    chain, in ascending order, and its score; chain_all(ssps, min_score=S) returns every chain scoring >= S (DESIGN.md section
+    20); get_dp() returns f and p of every SSP."""
 
     def __init__(self, stream=None, device_id=0, allocator=None):
         self._args = CallArgs(stream, allocator)
@@ -407,6 +430,24 @@ class SspChainer:
         ValueError."""
         D = _penalty("diag_penalty", diag_penalty)
         A = _penalty("anti_penalty", anti_penalty)
+        self._call(ssps, n, lambda addr, m: lib().gwb200_ssp_chainer_chain_device(self._h, C.c_void_p(addr), C.c_int32(m), C.c_int32(D),
+                                                                                  C.c_int32(A)))
+        return self.get_chain()
+
+    def chain_all(self, ssps, n=None, diag_penalty=0, anti_penalty=0, min_score=INT64_MIN):
+        """Every chain scoring >= min_score (DESIGN.md section 20.1; the default reports every chain): (int64 scores, int64
+        offsets of len(scores) + 1, int32 members), chain c being members[offsets[c]:offsets[c + 1]] in ascending index, the
+        chains in their heads' priority order. Takes the inputs of chain(); min_score is any int64. get_chain() then gives the
+        union of the chains' SSPs and the sum of their scores."""
+        D = _penalty("diag_penalty", diag_penalty)
+        A = _penalty("anti_penalty", anti_penalty)
+        S = _min_score("min_score", min_score)
+        self._call(ssps, n, lambda addr, m: lib().gwb200_ssp_chainer_chain_all_device(self._h, C.c_void_p(addr), C.c_int32(m), C.c_int32(D),
+                                                                                      C.c_int32(A), C.c_int64(S)))
+        return self.get_chains()
+
+    def _call(self, ssps, n, enqueue):
+        """Puts ssps (any form chain() takes) on the device, enqueues one call through enqueue(address, n) and finishes it."""
         keep = None
         if isinstance(ssps, np.ndarray):
             import torch
@@ -425,7 +466,7 @@ class SspChainer:
             addr = int(ssps or 0)
         if int(n) < 0:
             raise ValueError("n must be >= 0")
-        rc = check(lib().gwb200_ssp_chainer_chain_device(self._h, C.c_void_p(addr), C.c_int32(int(n)), C.c_int32(D), C.c_int32(A)))
+        rc = check(enqueue(addr, int(n)))
         if rc == invalid_input:
             raise ValueError("invalid chain arguments")
         if rc == invalid_operation:
@@ -435,7 +476,6 @@ class SspChainer:
         if rc == invalid_input:
             raise ValueError("an SSP length is below -1")
         self._n = int(n)
-        return self.get_chain()
 
     def get_chain(self):
         """(int32 SSP indices of the chain in ascending order, score) of the last call."""
@@ -444,6 +484,17 @@ class SspChainer:
         score = C.c_int64()
         check(lib().gwb200_ssp_chainer_get_chain(self._h, idx.ctypes.data_as(C.c_void_p), C.byref(score)))
         return idx, score.value
+
+    def get_chains(self):
+        """(scores, offsets, members) of the last call, as chain_all returns them; after chain() one chain, or none for n = 0."""
+        m = check(lib().gwb200_ssp_chainer_num_chains(self._h))
+        size = check(lib().gwb200_ssp_chainer_num_chained(self._h))
+        scores = np.zeros(m, dtype=np.int64)
+        offsets = np.zeros(m + 1, dtype=np.int64)
+        members = np.zeros(size, dtype=np.int32)
+        check(lib().gwb200_ssp_chainer_get_chains(self._h, scores.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p),
+                                                  members.ctypes.data_as(C.c_void_p)))
+        return scores, offsets, members
 
     def get_dp(self):
         """(f as int64, p as int32, -1 for none) of every SSP of the last call, by SSP index."""
@@ -506,12 +557,13 @@ def _records(seqs):
 class GenomeAligner:
     """The aligner with fixed parameters; run(targets, queries) aligns every query record against every target record."""
 
-    def __init__(self, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, round_anchors=0, chain=None, **params):
+    def __init__(self, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, round_anchors=0, chain=None,
+                 min_chain_score=None, **params):
         from ._lib import GenomeAlignerParams
         if strand not in STRANDS:
             raise ValueError("strand must be one of %s" % ", ".join(STRANDS))
         skip = _skip_args(skip_covered, round_anchors)
-        penalties = _chain_arg(chain)
+        penalties, min_score = _chain_args(chain, min_chain_score)
         p = default_genome_params()
         unknown = set(params) - set(p)
         if unknown:
@@ -537,12 +589,15 @@ class GenomeAligner:
         if skip[0]:
             check(lib().gwb200_genome_aligner_set_skip_covered(self._h, C.c_int32(skip[0]), C.c_int32(skip[1])))
         if penalties is not None:
-            self.set_chain(penalties)
+            self.set_chain(penalties, min_score)
 
-    def set_chain(self, chain):
-        """Chaining for later runs (DESIGN.md section 19): None or False turns it off, True or (D, A) turns it on."""
-        penalties = _chain_arg(chain)
+    def set_chain(self, chain, min_chain_score=None):
+        """Chaining for later runs (DESIGN.md section 19): None or False turns it off, True or (D, A) turns it on. With
+        min_chain_score=S (any int64; it needs chain) every chain scoring >= S goes to the gapped stage instead of the best one
+        (DESIGN.md section 20)."""
+        penalties, min_score = _chain_args(chain, min_chain_score)
         check(lib().gwb200_genome_aligner_set_chain(self._h, int(penalties is not None), *(C.c_int32(v) for v in penalties or (0, 0))))
+        check(lib().gwb200_genome_aligner_set_chain_min_score(self._h, int(min_score is not None), C.c_int64(min_score or 0)))
 
     def run(self, targets, queries):
         """-> (GENOME_DTYPE records, CIGAR strings, '' where has_cigar is 0). Blocking."""
@@ -584,6 +639,12 @@ class GenomeAligner:
         check(lib().gwb200_genome_aligner_last_chain_stats(self._h, C.byref(st)))
         return {name: getattr(st, name) for name in CHAIN_STATS}
 
+    def last_chain_count(self):
+        """The number of chains the last run reported, summed over every pair and strand (DESIGN.md section 20)."""
+        n = C.c_int64()
+        check(lib().gwb200_genome_aligner_last_chain_count(self._h, C.byref(n)))
+        return n.value
+
     def close(self):
         if self._h:
             lib().gwb200_genome_aligner_destroy(self._h)
@@ -596,15 +657,17 @@ class GenomeAligner:
             pass
 
 
-def align_genomes(targets, queries, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, chain=None, **params):
+def align_genomes(targets, queries, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, chain=None,
+                  min_chain_score=None, **params):
     """Aligns every query record against every target record on the plus strand, the minus strand or both. targets and queries
     are lists of sequences (str or int8 codes). Keyword parameters override gwb200_genome_aligner_default_params: score_matrix,
     xdrop, ssp_threshold, gap_open, gap_extend, ydrop, gapped_threshold, transition, block_size, traceback_budget. Returns
     (GENOME_DTYPE records, CIGAR strings); query coordinates are forward for both strands and minus-strand CIGARs read the
     target forward. Bad parameters raise ValueError before any device work. skip_covered=True does not extend the anchors that
     lie on an alignment kept earlier for the same pair and strand (DESIGN.md section 18). chain=True or (D, A) extends only the
-    SSPs of the highest-scoring colinear chain of each pair and strand (DESIGN.md section 19)."""
-    al = GenomeAligner(strand, stream, device_id, allocator, skip_covered, chain=chain, **params)
+    SSPs of the highest-scoring colinear chain of each pair and strand (DESIGN.md section 19); with min_chain_score=S as well,
+    those of every chain scoring >= S (DESIGN.md section 20)."""
+    al = GenomeAligner(strand, stream, device_id, allocator, skip_covered, chain=chain, min_chain_score=min_chain_score, **params)
     try:
         return al.run(targets, queries)
     finally:

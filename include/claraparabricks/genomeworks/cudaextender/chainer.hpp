@@ -44,12 +44,32 @@ public:
     /// Finishes the pending call; invalid_input when an SSP length is below -1.
     StatusType sync() { return static_cast<StatusType>(detail::check(gwb200_ssp_chainer_sync(h_))); }
 
-    /// The chain's SSP indices in ascending order, and its score, after sync().
+    /// Every chain scoring >= min_score (DESIGN.md section 20.1; any int64), on the chainer's stream, with the checks and
+    /// pending rules of chain_device.
+    StatusType chain_all_device(const ScoredSegmentPair* d_ssps, int32_t n, int32_t diag_penalty, int32_t anti_penalty, int64_t min_score)
+    {
+        return static_cast<StatusType>(detail::check(gwb200_ssp_chainer_chain_all_device(h_, d_ssps, n, diag_penalty, anti_penalty, min_score)));
+    }
+
+    /// The chain's SSP indices in ascending order, and its score, after sync(); after chain_all_device, the union of the
+    /// reported chains and the sum of their scores.
     std::vector<int32_t> get_chain(int64_t& score) const
     {
         std::vector<int32_t> out(static_cast<std::size_t>(detail::check(gwb200_ssp_chainer_num_chained(h_))));
         detail::check(gwb200_ssp_chainer_get_chain(h_, out.data(), &score));
         return out;
+    }
+
+    /// The reported chains after sync(), in their heads' priority order: their scores, offsets (one more than the chains) and,
+    /// returned, their members, chain c's SSP indices ascending in [offsets[c], offsets[c + 1]).
+    std::vector<int32_t> get_chains(std::vector<int64_t>& scores, std::vector<int64_t>& offsets) const
+    {
+        const int32_t chains = detail::check(gwb200_ssp_chainer_num_chains(h_));
+        std::vector<int32_t> members(static_cast<std::size_t>(detail::check(gwb200_ssp_chainer_num_chained(h_))));
+        scores.assign(static_cast<std::size_t>(chains), 0);
+        offsets.assign(static_cast<std::size_t>(chains) + 1, 0);
+        detail::check(gwb200_ssp_chainer_get_chains(h_, scores.data(), offsets.data(), members.data()));
+        return members;
     }
 
 private:

@@ -528,6 +528,20 @@ int gwb200_ssp_chainer_get_chain(const gwb200_ssp_chainer* chainer, int32_t* ind
 int gwb200_ssp_chainer_get_dp(const gwb200_ssp_chainer* chainer, int64_t* f, int32_t* p);
 /* Device ms of the last finished call (CUDA events; -1 when not available). */
 int gwb200_ssp_chainer_last_ms(const gwb200_ssp_chainer* chainer, float* ms);
+/* Every chain above a minimum score (DESIGN.md section 20.1): the DP above, then the SSPs in priority order (f descending,
+ * ties to the smallest index); each SSP h not yet claimed heads a candidate chain h, p(h), p(p(h)), ... up to -1 or the first
+ * SSP already claimed, all of which it claims. A candidate's score is that of its members alone (sum of s less the links'
+ * penalties, = f(h) - f(c_1) + s(c_1) for its first member c_1); it is reported when score >= min_score (any int64). Chains
+ * not reported keep their SSPs claimed. Same checks and pending rules as chain_device. After sync(), num_chained and
+ * get_chain give the union of the reported chains' SSPs in ascending index and the sum of their scores; get_dp and last_ms are
+ * as above. */
+int gwb200_ssp_chainer_chain_all_device(gwb200_ssp_chainer* chainer, const void* d_ssps, int32_t n, int32_t diag_penalty, int32_t anti_penalty,
+                                        int64_t min_score);
+/* After sync(): the reported chains, in their heads' priority order (one chain after chain_device, none when n = 0). scores
+ * [num_chains], offsets [num_chains + 1] (offsets[0] = 0) and members [offsets[num_chains]]: chain c's SSP indices, ascending,
+ * are members[offsets[c], offsets[c + 1]). get_chains returns num_chains. Without a finished call => GWB200_E_RUNTIME. */
+int32_t gwb200_ssp_chainer_num_chains(const gwb200_ssp_chainer* chainer);
+int gwb200_ssp_chainer_get_chains(const gwb200_ssp_chainer* chainer, int64_t* scores, int64_t* offsets, int32_t* members);
 
 /* ------------------------------------------------------------------------------------------------
  * cudaextender, genome-to-genome aligner (DESIGN.md section 17): every (target record, query record) pair on the plus strand,
@@ -614,8 +628,17 @@ typedef struct gwb200_chain_stats
     int64_t pairs;        /* (pair, strand)s chained: those with at least one SSP */
     double chain_ms;      /* device ms of the chainer */
 } gwb200_chain_stats;
-/* Of the last run, summed over every pair and strand (all zero with chaining off). */
+/* Of the last run, summed over every pair and strand (all zero with chaining off). With all chains on, ssps_chained is the
+ * size of the union of the reported chains. */
 int gwb200_genome_aligner_last_chain_stats(const gwb200_genome_aligner* aligner, gwb200_chain_stats* out);
+/* All chains (DESIGN.md section 20), off by default; it holds for later runs until turned off. While chaining is on
+ * (set_chain), on != 0 sends the union of every chain scoring >= min_score (gwb200_ssp_chainer_chain_all_device) of each
+ * (pair, strand) to the gapped stage instead of the best chain; while chaining is off it changes nothing. Every min_score is
+ * valid. */
+int gwb200_genome_aligner_set_chain_min_score(gwb200_genome_aligner* aligner, int32_t on, int64_t min_score);
+/* The number of chains the last run reported, summed over every pair and strand (one per chained (pair, strand) with the best
+ * chain; zero with chaining off). */
+int gwb200_genome_aligner_last_chain_count(const gwb200_genome_aligner* aligner, int64_t* chains);
 
 /* ------------------------------------------------------------------------------------------------
  * cudamapper (minimizer index)

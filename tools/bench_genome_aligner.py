@@ -2,7 +2,8 @@
 matrix, LASTZ-style gapped parameters, blocks of 2^25 seeds).
 
     python tools/bench_genome_aligner.py [--steps K] [--warmup W] [--workloads sample,assembly]
-                                         [--modes default,skip,chain,chain+skip] [--skip-covered]
+                                         [--modes default,skip,chain,chain+skip,chains,chains+skip] [--skip-covered]
+                                         [--min-chain-score 30000]
 
 Workloads:
   sample    the golden sample (one 250 kb record) against itself;
@@ -19,7 +20,11 @@ after `warmup`). The card name and power limit are read in the same run. Writes 
 line per mode; skip is the skip-covered mode (DESIGN.md section 18). A skip line adds the skip stats of the gapped stage and
 whether every skip-mode alignment's score, records, strand and intervals are among the default mode's (subset_of_default,
 when both modes ran). --skip-covered is --modes skip. chain is chaining with zero penalties (DESIGN.md section 19) and
-chain+skip chaining in skip-covered mode; their lines add the chain stats (SSPs in, SSPs chained, pairs, chain ms).
+chain+skip chaining in skip-covered mode; their lines add the chain stats (SSPs in, SSPs chained, pairs, chain ms). chains is
+every chain scoring >= --min-chain-score (DESIGN.md section 20; default 30,000, ten times the SSP threshold) and chains+skip
+that in skip-covered mode; their lines add the chain stats and the number of chains. On the assembly workload every line
+reports pieces_found: the pieces that one alignment on their strand overlaps for at least half of their length in both
+sequences, and the pieces it misses.
 """
 import argparse
 import json
@@ -47,19 +52,37 @@ def card():
 
 
 def assembly(seed=2026, target_len=10_000_000, pieces=80):
+    """([target], [query], counts, placements): each placement is (query begin, query end, target begin, target end, strand)
+    of one piece, strand 1 for a reverse-complemented piece."""
     import seeder_libs as sl
     rng = np.random.default_rng(seed)
     target = rng.integers(0, 4, target_len).astype(np.int8)
-    parts, rc = [], 0
+    parts, rc, placed, at = [], 0, [], 0
     for _ in range(pieces):
         n = int(rng.integers(5000, 50001))
         s = int(rng.integers(0, target_len - n))
         piece = sl.mutate(target[s:s + n], float(rng.uniform(0.02, 0.10)), rng)
+        strand = 0
         if rng.random() < 1 / 3:
             piece = sl.reverse_complement(piece)
             rc += 1
+            strand = 1
         parts.append(piece)
-    return [target], [np.concatenate(parts)], dict(pieces=pieces, reverse_complemented=rc)
+        placed.append((at, at + len(piece), s, s + n, strand))
+        at += len(piece)
+    return [target], [np.concatenate(parts)], dict(pieces=pieces, reverse_complemented=rc), placed
+
+
+def pieces_found(rec, placed):
+    """Indices of the pieces that one alignment on their strand overlaps for at least half of their length in both sequences."""
+    found = []
+    for k, (qb, qe, tb, te, strand) in enumerate(placed):
+        mine = rec[rec["strand"] == strand]
+        oq = np.minimum(mine["query_end"].astype(np.int64), qe) - np.maximum(mine["query_begin"].astype(np.int64), qb)
+        ot = np.minimum(mine["target_end"].astype(np.int64), te) - np.maximum(mine["target_begin"].astype(np.int64), tb)
+        if ((2 * oq >= qe - qb) & (2 * ot >= te - tb)).any():
+            found.append(k)
+    return found
 
 
 def key(r):
@@ -67,9 +90,10 @@ def key(r):
                                      "target_end"))
 
 
-def run(name, targets, queries, steps, warmup, extra, modes=("default",)):
+def run(name, targets, queries, steps, warmup, extra, modes=("default",), min_chain_score=30000, placed=None):
     from genomeworks_b200 import cudaextender as ce
-    aligners = {m: ce.GenomeAligner(skip_covered=m in ("skip", "chain+skip"), chain=m in ("chain", "chain+skip")) for m in modes}
+    aligners = {m: ce.GenomeAligner(skip_covered=m.endswith("skip"), chain=m.startswith("chain"),
+                                    min_chain_score=min_chain_score if m.startswith("chains") else None) for m in modes}
     for _ in range(warmup):
         for al in aligners.values():
             al.run(targets, queries)
@@ -83,8 +107,15 @@ def run(name, targets, queries, steps, warmup, extra, modes=("default",)):
     for m, al in aligners.items():
         ms, counts = al.last_stats()
         more = dict(extra, mode=m)
-        if m in ("chain", "chain+skip"):
+        if m.startswith("chain"):
             more["chain_stats"] = al.last_chain_stats()
+            more["chains"] = al.last_chain_count()
+        if m.startswith("chains"):
+            more["min_chain_score"] = min_chain_score
+        if placed is not None:
+            found = pieces_found(out[m], placed)
+            more["pieces_found"] = len(found)
+            more["pieces_missed"] = [k for k in range(len(placed)) if k not in found]
         if m == "skip":
             more["skip_stats"] = al.last_skip_stats()
             if "default" in out:
@@ -114,10 +145,11 @@ def main():
     ap.add_argument("--workloads", default="sample,assembly")
     ap.add_argument("--modes", default="default")
     ap.add_argument("--skip-covered", action="store_true")
+    ap.add_argument("--min-chain-score", type=int, default=30000)
     a = ap.parse_args()
     modes = ["skip"] if a.skip_covered else a.modes.split(",")
-    if set(modes) - {"default", "skip", "chain", "chain+skip"}:
-        sys.exit("modes are default, skip, chain and chain+skip")
+    if set(modes) - {"default", "skip", "chain", "chain+skip", "chains", "chains+skip"}:
+        sys.exit("modes are default, skip, chain, chain+skip, chains and chains+skip")
     import torch
     if not torch.cuda.is_available():
         sys.exit("bench_genome_aligner.py needs a CUDA device")
@@ -125,10 +157,10 @@ def main():
         if w == "sample":
             import extender_libs as xl
             seq, _, _ = xl.sample()
-            run("sample", [seq], [seq], a.steps, a.warmup, {}, modes)
+            run("sample", [seq], [seq], a.steps, a.warmup, {}, modes, a.min_chain_score)
         elif w == "assembly":
-            t, q, extra = assembly()
-            run("assembly", t, q, a.steps, a.warmup, extra, modes)
+            t, q, extra, placed = assembly()
+            run("assembly", t, q, a.steps, a.warmup, extra, modes, a.min_chain_score, placed)
         else:
             sys.exit("unknown workload " + w)
 

@@ -57,6 +57,9 @@ namespace
         --chain[=D,A]
             extend only the highest-scoring colinear chain of ungapped segments of each record pair and strand; D and A
             are the diagonal and anti-diagonal gap penalties of the chain, each in [0, 1048576] [0,0]
+        --chain-min-score=S
+            with --chain, extend the SSPs of every colinear chain scoring at least S (any 64-bit integer) instead of the
+            best chain only
         -h, --help
             this text
         -v, --version
@@ -144,14 +147,16 @@ int main(int argc, char* argv[])
         {"gap-extend", required_argument, 0, 'e'},      {"gapped-threshold", required_argument, 0, 'g'},
         {"block-size", required_argument, 0, 'B'},      {"traceback-budget", required_argument, 0, 'b'},
         {"skip-covered", no_argument, 0, 257},          {"chain", optional_argument, 0, 258},
+        {"chain-min-score", required_argument, 0, 259},
         {"version", no_argument, 0, 'v'},               {"help", no_argument, 0, 'h'},
         {0, 0, 0, 0},
     };
     gwb200_genome_aligner_params p;
     gwb200_genome_aligner_default_params(&p);
     const int64_t i32 = INT32_MAX;
-    bool skip_covered = false, chain = false;
+    bool skip_covered = false, chain = false, chain_all = false;
     int32_t chain_pen[2] = {0, 0};
+    int64_t chain_min    = 0;
     int argument      = 0;
     while ((argument = getopt_long(argc, argv, "s:x:T:y:o:e:g:B:b:vh", options, nullptr)) != -1)
     {
@@ -191,6 +196,10 @@ int main(int argc, char* argv[])
             chain_pen[1] = static_cast<int32_t>(to_int(s.substr(comma + 1).c_str(), "chain's anti-diagonal penalty", 0, 1 << 20));
             break;
         }
+        case 259:
+            chain_all = true;
+            chain_min = to_int(optarg, "chain-min-score", INT64_MIN, INT64_MAX);
+            break;
         case 'x': p.xdrop = static_cast<int32_t>(to_int(optarg, "xdrop", 0, i32)); break;
         case 'T': p.ssp_threshold = static_cast<int32_t>(to_int(optarg, "ssp-threshold", -i32 - 1, i32)); break;
         case 'y': p.ydrop = static_cast<int32_t>(to_int(optarg, "ydrop", 0, 1 << 28)); break;
@@ -203,6 +212,11 @@ int main(int argc, char* argv[])
         case 'h': help(0);
         default: std::exit(1);
         }
+    }
+    if (chain_all && !chain)
+    {
+        std::cerr << "ERROR: --chain-min-score needs --chain" << std::endl;
+        std::exit(1);
     }
     if (optind + 2 != argc)
     {
@@ -223,6 +237,8 @@ int main(int argc, char* argv[])
         fail("could not set the skip-covered mode");
     if (chain && gwb200_genome_aligner_set_chain(a, 1, chain_pen[0], chain_pen[1]) != 0)
         fail("could not set chaining");
+    if (chain_all && gwb200_genome_aligner_set_chain_min_score(a, 1, chain_min) != 0)
+        fail("could not set the minimum chain score");
     const int rc = gwb200_genome_aligner_run(a, tcodes.data(), toff.data(), static_cast<int32_t>(targets.size()), qcodes.data(), qoff.data(),
                                              static_cast<int32_t>(queries.size()));
     if (rc != 0)
