@@ -26,7 +26,8 @@ struct gwb200_extender
     cudaStream_t stream = nullptr;
     int32_t xdrop      = 0;
     int32_t no_entropy = 0;
-    int32_t grid_max   = 0; // resident CTAs of the extension kernel on this device
+    bool wide          = false; // the extension kernel's sums are int64 (narrow_scores_suffice is false for the matrix and xdrop)
+    int32_t grid_max   = 0;     // resident CTAs of the extension kernel on this device
     int32_t n_sms      = 0;
     MemHooks hooks;
 
@@ -122,9 +123,9 @@ int extension_launch(const gwb200_extender* e, const int8_t* query, int32_t qlen
     if (n == 0)
         return 0;
     const int32_t grid = static_cast<int32_t>(std::min<int64_t>(e->grid_max, (static_cast<int64_t>(n) + kWarpsPerCta - 1) / kWarpsPerCta));
-    ungapped_xdrop_kernel<<<grid, kWarpsPerCta * 32, 0, e->stream>>>(target, tlen, query, qlen, e->sub_d.p, e->no_entropy, e->xdrop,
-                                                                      score_threshold, static_cast<const SeedPairD*>(seeds), n,
-                                                                      static_cast<SspD*>(kept), num_kept, examined);
+    auto kernel        = e->wide ? ungapped_xdrop_kernel<int64_t> : ungapped_xdrop_kernel<int32_t>;
+    kernel<<<grid, kWarpsPerCta * 32, 0, e->stream>>>(target, tlen, query, qlen, e->sub_d.p, e->no_entropy, e->xdrop, score_threshold,
+                                                      static_cast<const SeedPairD*>(seeds), n, static_cast<SspD*>(kept), num_kept, examined);
     GWB200_CUDA_TRY(cudaGetLastError());
     count_launch(1);
     return 0;
@@ -199,10 +200,12 @@ int gwb200_extender_create_with_allocator(gwb200_extender** out, const int32_t* 
     e->stream          = static_cast<cudaStream_t>(stream);
     e->xdrop           = xdrop_threshold;
     e->no_entropy      = no_entropy ? 1 : 0;
+    e->wide            = !narrow_scores_suffice(score_mat, xdrop_threshold);
     e->hooks           = MemHooks(alloc_fn, free_fn, user);
     int per_sm = 0;
     cudaDeviceGetAttribute(&e->n_sms, cudaDevAttrMultiProcessorCount, device_id);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ungapped_xdrop_kernel, kWarpsPerCta * 32, 0);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, e->wide ? ungapped_xdrop_kernel<int64_t> : ungapped_xdrop_kernel<int32_t>,
+                                                  kWarpsPerCta * 32, 0);
     e->grid_max = std::max(1, e->n_sms * per_sm);
     if (!e->sub_d.ensure(kNuc * kNuc))
     {

@@ -69,22 +69,42 @@ __device__ __forceinline__ int byte_of(const uint32_t (&w)[kPosPerLane / 4], int
 
 struct ExtResult
 {
-    int32_t max_score; // best prefix score (0 when no position beats the start value)
+    int64_t max_score; // best prefix score (0 when no position beats the start value)
     int32_t max_pos;   // its offset (the start value's offset when none does)
 };
+
+// The score type of the sums inside one step. int32 holds them when every value a step computes relative to the sum at its
+// start stays in range: the step's partial sums lie in [-kTile * M, kTile * M] for M = max |matrix entry|, the running maximum
+// enters the step at most xdrop above that sum, so the X-drop difference is at most max(xdrop, kTile * M) + kTile * M
+// (DESIGN.md 9.2). Otherwise the kernel runs on int64, which holds any sum of fewer than 2^31 int32 entries.
+inline bool narrow_scores_suffice(const int32_t* sub, int32_t xdrop)
+{
+    int64_t m = 0;
+    for (int i = 0; i < kNuc * kNuc; ++i)
+    {
+        const int64_t a = sub[i] < 0 ? -static_cast<int64_t>(sub[i]) : sub[i];
+        m               = a > m ? a : m;
+    }
+    const int64_t span = static_cast<int64_t>(kTile) * m;
+    return (xdrop > span ? static_cast<int64_t>(xdrop) : span) + span <= INT32_MAX;
+}
 
 // One direction of the extension. Right (kLeft == false): offsets 0, 1, ... at seed + offset, maximum starts at (0, -1).
 // Left (kLeft == true): offsets 1, 2, ... at seed - offset, maximum starts at (0, 0). `limit` = number of offsets that lie in
 // both sequences. A position becomes the maximum only when strictly greater (ties keep the earliest); the extension stops at
 // the first offset whose score is more than xdrop below the running maximum (that offset is excluded) or at the limit.
-template <bool kLeft>
+// The sum is carried from step to step as int64; inside a step the sums and the maximum are ScoreT, relative to the sum at the
+// step's start (narrow_scores_suffice says when int32 is enough).
+template <bool kLeft, typename ScoreT>
 __device__ __forceinline__ ExtResult extend_one_side(const int8_t* __restrict__ target, int64_t tlen, const int8_t* __restrict__ query,
                                                      int64_t qlen, int64_t tseed, int64_t qseed, int64_t limit, const int32_t* sub,
                                                      int32_t xdrop, int64_t& examined)
 {
     const int lane  = threadIdx.x & 31;
     const int first = kLeft ? 1 : 0;
-    int32_t carry_s = 0, carry_m = 0, carry_p = kLeft ? 0 : -1;
+    int64_t carry_s = 0;      // the sum at the step's start
+    ScoreT carry_m  = 0;      // the maximum so far, relative to carry_s: in [0, xdrop], since the step's start did not drop
+    int32_t carry_p = kLeft ? 0 : -1;
     for (int64_t base = 0;; base += kTile)
     {
         const int64_t o0 = base + first + static_cast<int64_t>(lane) * kPosPerLane; // offset of this lane's first position
@@ -100,8 +120,9 @@ __device__ __forceinline__ ExtResult extend_one_side(const int8_t* __restrict__ 
             load_window(query, qlen, qseed + o0, qw);
         }
         // lane-local prefix sums and (max, first argmax)
-        int32_t s[kPosPerLane];
-        int32_t run = 0, lmax = INT_MIN, larg = 0;
+        ScoreT s[kPosPerLane];
+        ScoreT run = 0, lmax = 0;
+        int32_t larg = 0;
 #pragma unroll
         for (int j = 0; j < kPosPerLane; ++j)
         {
@@ -109,29 +130,29 @@ __device__ __forceinline__ ExtResult extend_one_side(const int8_t* __restrict__ 
             const bool in  = kLeft ? (o0 + j <= limit) : (o0 + j < limit);
             run += in ? sub[byte_of(tw, bj) * kNuc + byte_of(qw, bj)] : 0;
             s[j] = run;
-            if (run > lmax)
+            if (j == 0 || run > lmax)
             {
                 lmax = run;
                 larg = j;
             }
         }
         // warp prefix sum of the lane totals
-        int32_t incl = run;
+        ScoreT incl = run;
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1)
         {
-            const int32_t v = __shfl_up_sync(0xffffffffu, incl, d);
+            const ScoreT v = __shfl_up_sync(0xffffffffu, incl, d);
             if (lane >= d)
                 incl += v;
         }
-        const int32_t lane_base = carry_s + incl - run;
+        const ScoreT lane_base = incl - run;
         // warp (max, first argmax) scan: ties go to the earlier lane
-        int32_t m = lane_base + lmax;
+        ScoreT m  = lane_base + lmax;
         int32_t p = static_cast<int32_t>(o0) + larg;
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1)
         {
-            const int32_t om = __shfl_up_sync(0xffffffffu, m, d);
+            const ScoreT om  = __shfl_up_sync(0xffffffffu, m, d);
             const int32_t op = __shfl_up_sync(0xffffffffu, p, d);
             if (lane >= d && om >= m)
             {
@@ -139,7 +160,7 @@ __device__ __forceinline__ ExtResult extend_one_side(const int8_t* __restrict__ 
                 p = op;
             }
         }
-        int32_t run_m = __shfl_up_sync(0xffffffffu, m, 1);
+        ScoreT run_m  = __shfl_up_sync(0xffffffffu, m, 1);
         int32_t run_p = __shfl_up_sync(0xffffffffu, p, 1);
         if (lane == 0 || !(run_m > carry_m))
         {
@@ -147,12 +168,13 @@ __device__ __forceinline__ ExtResult extend_one_side(const int8_t* __restrict__ 
             run_p = carry_p;
         }
         // walk this lane's positions from the maximum before it: first X-drop
-        bool dropped = false;
-        int32_t drop_m = 0, drop_p = 0;
+        bool dropped  = false;
+        ScoreT drop_m = 0;
+        int32_t drop_p = 0;
 #pragma unroll
         for (int j = 0; j < kPosPerLane; ++j)
         {
-            const int32_t sj = lane_base + s[j];
+            const ScoreT sj = lane_base + s[j];
             if (sj > run_m)
             {
                 run_m = sj;
@@ -171,18 +193,22 @@ __device__ __forceinline__ ExtResult extend_one_side(const int8_t* __restrict__ 
         if (drops)
         {
             const int src = __ffs(drops) - 1;
-            return ExtResult{__shfl_sync(0xffffffffu, drop_m, src), __shfl_sync(0xffffffffu, drop_p, src)};
+            return ExtResult{carry_s + __shfl_sync(0xffffffffu, drop_m, src), __shfl_sync(0xffffffffu, drop_p, src)};
         }
         carry_m = __shfl_sync(0xffffffffu, run_m, 31);
         carry_p = __shfl_sync(0xffffffffu, run_p, 31);
         if (in_tile <= kTile)
-            return ExtResult{carry_m, carry_p};
-        carry_s = __shfl_sync(0xffffffffu, lane_base + s[kPosPerLane - 1], 31);
+            return ExtResult{carry_s + carry_m, carry_p};
+        const ScoreT step_sum = __shfl_sync(0xffffffffu, lane_base + s[kPosPerLane - 1], 31);
+        carry_s += step_sum;
+        carry_m -= step_sum;
     }
 }
 
 // Extends every seed; a kept segment is appended to `kept` at an index taken from `*num_kept`. Seeds that do not lie inside
-// both sequences produce nothing. `examined` accumulates the positions the extensions covered.
+// both sequences produce nothing. `examined` accumulates the positions the extensions covered. ScoreT: see
+// narrow_scores_suffice.
+template <typename ScoreT>
 __global__ void __launch_bounds__(kWarpsPerCta * 32) ungapped_xdrop_kernel(
     const int8_t* __restrict__ target, int32_t tlen, const int8_t* __restrict__ query, int32_t qlen, const int32_t* __restrict__ sub_mat,
     int32_t no_entropy, int32_t xdrop, int32_t score_threshold, const SeedPairD* __restrict__ seeds, int32_t n, SspD* __restrict__ kept,
@@ -202,12 +228,13 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) ungapped_xdrop_kernel(
         const int64_t ts = sp.target, qs = sp.query;
         if (ts >= tlen || qs >= qlen)
             continue;
-        const ExtResult r = extend_one_side<false>(target, tlen, query, qlen, ts, qs, min(tlen - ts, qlen - qs), sub, xdrop, examined);
-        const ExtResult l = extend_one_side<true>(target, tlen, query, qlen, ts, qs, min(ts, qs), sub, xdrop, examined);
-        const int32_t total  = r.max_score + l.max_score;
+        const ExtResult r =
+            extend_one_side<false, ScoreT>(target, tlen, query, qlen, ts, qs, min(tlen - ts, qlen - qs), sub, xdrop, examined);
+        const ExtResult l = extend_one_side<true, ScoreT>(target, tlen, query, qlen, ts, qs, min(ts, qs), sub, xdrop, examined);
+        const int64_t total  = r.max_score + l.max_score; // >= 0
         const int32_t length = r.max_pos + l.max_pos;
-        double entropy       = 1.0;
-        if (!no_entropy && total >= score_threshold && total <= 3 * score_threshold)
+        int64_t score        = total;
+        if (!no_entropy && total >= score_threshold && total <= 3 * static_cast<int64_t>(score_threshold))
         {
             // per-base counts of the matching A/C/G/T positions inside the final segment (length + 1 positions)
             int32_t cnt[kNucEntropy] = {0, 0, 0, 0};
@@ -237,14 +264,14 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) ungapped_xdrop_kernel(
                         acc             = fma(pr, log(pr), acc);
                     }
                 }
-                entropy = -acc / kLn4;
+                score = static_cast<int64_t>(static_cast<double>(total) * (-acc / kLn4)); // total <= 3T < 2^33: exact
             }
         }
-        const int32_t score = static_cast<int32_t>(static_cast<double>(total) * entropy);
         if (lane == 0 && score >= score_threshold)
         {
             const int32_t slot = atomicAdd(num_kept, 1);
-            kept[slot] = SspD{static_cast<uint32_t>(qs - l.max_pos), static_cast<uint32_t>(ts - l.max_pos), length, score};
+            kept[slot] = SspD{static_cast<uint32_t>(qs - l.max_pos), static_cast<uint32_t>(ts - l.max_pos), length,
+                              static_cast<int32_t>(score < INT32_MAX ? score : INT32_MAX)};
         }
     }
     if (lane == 0 && examined)

@@ -342,7 +342,8 @@ float gwb200_global_aligner_last_kernel_ms(gwb200_global_aligner* aligner);
  *                                                                                   create_extender)
  * Seeds are SeedPair records {uint32 query_position_in_read; uint32 target_position_in_read} and results ScoredSegmentPair
  * records {SeedPair start_coord; int32 length; int32 score} (16 bytes), passed as void pointers. Sequences are encoded as in
- * cudaextender/utils.hpp (A=0 C=1 G=2 T=3, lowercase acgt=4, n/N=5, other=6, '&'=7); other codes are read modulo 8.
+ * cudaextender/utils.hpp (A=0 C=1 G=2 T=3, lowercase acgt=4, n/N=5, other=6, '&'=7); other codes are read modulo 8. Scores
+ * are computed exactly in int64 at any matrix entry and length; a score above INT32_MAX is reported as INT32_MAX.
  * ---------------------------------------------------------------------------------------------- */
 
 /* cudaextender::StatusType, cudaextender.hpp */

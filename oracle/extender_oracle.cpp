@@ -30,15 +30,17 @@ double do_log(double x) { return g_log ? g_log(x) : std::log(x); }
 
 struct Side
 {
-    int32_t max_score;
+    int64_t max_score;
     int32_t max_pos;
 };
 
-// Offsets first, first+1, ... while offset <= last; score of offset o = sub[target(o) * 8 + query(o)].
+// Offsets first, first+1, ... while offset <= last; score of offset o = sub[target(o) * 8 + query(o)]. The sums are int64:
+// a side has fewer than 2^31 offsets of |entry| <= 2^31, so |sum| < 2^62 and the X-drop difference never wraps.
 template <typename At>
 Side extend(int64_t first, int64_t last, int32_t start_pos, At at, int32_t xdrop)
 {
-    int32_t sum = 0, best = 0, best_pos = start_pos;
+    int64_t sum = 0, best = 0;
+    int32_t best_pos = start_pos;
     for (int64_t o = first; o <= last; ++o)
     {
         sum += at(o);
@@ -59,18 +61,19 @@ extern "C" {
 
 void oracle_extender_set_log(double (*fn)(double)) { g_log = fn; }
 
-// One seed: out = {query start, target start, length, score, kept, total}. The seed must lie inside both sequences.
-void oracle_extender_seed(const int8_t* query, int32_t qlen, const int8_t* target, int32_t tlen, const int32_t* sub, int32_t xdrop,
-                          int32_t no_entropy, int32_t score_threshold, uint32_t qs, uint32_t ts, int32_t* out)
+// One seed, exact: out = {query start, target start, length, score, kept, total}, score and total as int64 (DESIGN.md 9.1:
+// score = total unless the entropy rule applies, kept iff score >= threshold). The seed must lie inside both sequences.
+void oracle_extender_seed_wide(const int8_t* query, int32_t qlen, const int8_t* target, int32_t tlen, const int32_t* sub, int32_t xdrop,
+                               int32_t no_entropy, int32_t score_threshold, uint32_t qs, uint32_t ts, int64_t* out)
 {
     auto score_at = [&](int64_t tp, int64_t qp) { return sub[code(target[tp]) * 8 + code(query[qp])]; };
     const Side r = extend(0, std::min<int64_t>(tlen - ts, qlen - qs) - 1, -1, [&](int64_t o) { return score_at(ts + o, qs + o); }, xdrop);
     const Side l = extend(1, std::min<int64_t>(ts, qs), 0, [&](int64_t o) { return score_at(ts - o, qs - o); }, xdrop);
-    const int32_t total  = r.max_score + l.max_score;
+    const int64_t total  = r.max_score + l.max_score;
     const int32_t length = r.max_pos + l.max_pos;
     const int64_t t0 = static_cast<int64_t>(ts) - l.max_pos, q0 = static_cast<int64_t>(qs) - l.max_pos;
-    double entropy = 1.0;
-    if (!no_entropy && total >= score_threshold && total <= 3 * score_threshold)
+    int64_t score = total;
+    if (!no_entropy && total >= score_threshold && total <= 3 * static_cast<int64_t>(score_threshold))
     {
         int64_t count[4] = {0, 0, 0, 0};
         for (int64_t k = 0; k <= length; ++k)
@@ -90,16 +93,27 @@ void oracle_extender_seed(const int8_t* query, int32_t qlen, const int8_t* targe
                     acc            = std::fma(p, do_log(p), acc);
                 }
             }
-            entropy = -acc / static_cast<double>(std::log(4.0f));
+            const double entropy = -acc / static_cast<double>(std::log(4.0f));
+            score                = static_cast<int64_t>(static_cast<double>(total) * entropy); // total <= 3T < 2^33: exact
         }
     }
-    const int32_t score = static_cast<int32_t>(static_cast<double>(total) * entropy);
-    out[0] = static_cast<int32_t>(q0);
-    out[1] = static_cast<int32_t>(t0);
+    out[0] = q0;
+    out[1] = t0;
     out[2] = length;
     out[3] = score;
     out[4] = score >= score_threshold ? 1 : 0;
     out[5] = total;
+}
+
+// One seed as the engine reports it: out = {query start, target start, length, score, kept, total}, the score and the total
+// saturated at INT32_MAX (both are >= 0).
+void oracle_extender_seed(const int8_t* query, int32_t qlen, const int8_t* target, int32_t tlen, const int32_t* sub, int32_t xdrop,
+                          int32_t no_entropy, int32_t score_threshold, uint32_t qs, uint32_t ts, int32_t* out)
+{
+    int64_t w[6];
+    oracle_extender_seed_wide(query, qlen, target, tlen, sub, xdrop, no_entropy, score_threshold, qs, ts, w);
+    for (int k = 0; k < 6; ++k)
+        out[k] = static_cast<int32_t>(std::min<int64_t>(w[k], INT32_MAX));
 }
 
 // Stable sort by (uint32 diagonal target - query, target ascending, length descending, score descending), then keep each
