@@ -5,6 +5,9 @@
 // stable radix passes over all n slots (sort_unique) (secondary keys, then primary keys; slots of dropped seeds sort last) -> "first or not contained in
 // its predecessor" flags -> cub::DeviceSelect::Flagged, which writes the result count on the device. Nothing in it waits for
 // the device.
+//
+// The genome aligner calls the record-bounded extension kernel and sort_unique_groups instead (DESIGN.md section 21): a third,
+// most significant radix pass by record pair, and the unique rule within each record pair.
 
 #include "../../include/gwb200.h"
 #include "common.cuh"
@@ -28,6 +31,7 @@ struct gwb200_extender
     int32_t no_entropy = 0;
     bool wide          = false; // the extension kernel's sums are int64 (narrow_scores_suffice is false for the matrix and xdrop)
     int32_t grid_max   = 0;     // resident CTAs of the extension kernel on this device
+    int32_t grid_max_groups = 0; // the same for its record-bounded variant
     int32_t n_sms      = 0;
     MemHooks hooks;
 
@@ -37,6 +41,8 @@ struct gwb200_extender
     DevBuf<uint64_t> keys_a{&hooks}, keys_b{&hooks};
     DevBuf<uint32_t> idx_a{&hooks}, idx_b{&hooks};
     DevBuf<uint8_t> flags_d{&hooks};
+    DevBuf<SspD> local_d{&hooks};                            // sort_unique_groups: segments in record coordinates
+    DevBuf<uint64_t> pair_d{&hooks}, sorted_pair_d{&hooks}; // and their record pairs
     DevBuf<int32_t> num_kept_d{&hooks};
     DevBuf<unsigned long long> examined_d{&hooks};
     DevBuf<char> cub_d{&hooks};
@@ -66,6 +72,19 @@ int bits_for(int64_t v) // smallest b with v < 2^b
 
 int bad_alloc() { return set_error(GWB200_E_BAD_ALLOC, "Could not allocate device memory for the extender workspace"); }
 
+template <bool kBounded>
+auto extension_kernel(bool wide)
+{
+    return wide ? ungapped_xdrop_kernel<int64_t, kBounded> : ungapped_xdrop_kernel<int32_t, kBounded>;
+}
+
+int32_t resident_ctas(const void* kernel, int32_t n_sms)
+{
+    int per_sm = 0;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kWarpsPerCta * 32, 0);
+    return std::max(1, n_sms * per_sm);
+}
+
 // The sort and unique workspaces for `slots` kept segments.
 int ensure_sort(gwb200_extender* e, int32_t slots)
 {
@@ -81,33 +100,6 @@ int ensure_sort(gwb200_extender* e, int32_t slots)
     return 0;
 }
 
-// The device path of both extend calls; pointers and sizes are already checked.
-int run_extend(gwb200_extender* e, const int8_t* query, int32_t qlen, const int8_t* target, int32_t tlen, int32_t score_threshold,
-               const SeedPairD* seeds, int32_t n, SspD* out, int32_t* num_out)
-{
-    DeviceGuard guard(e->device_id);
-    e->launched = false;
-    if (n == 0)
-    {
-        GWB200_CUDA_TRY(cudaMemsetAsync(num_out, 0, sizeof(int32_t), e->stream));
-        return GWB200_EXT_SUCCESS;
-    }
-    if (!e->kept_d.ensure(n) || !e->num_kept_d.ensure(1) || !e->examined_d.ensure(1))
-        return bad_alloc();
-    if (const int rc = ensure_sort(e, n))
-        return rc;
-    GWB200_CUDA_TRY(cudaMemsetAsync(e->num_kept_d.p, 0, sizeof(int32_t), e->stream));
-    GWB200_CUDA_TRY(cudaMemsetAsync(e->examined_d.p, 0, sizeof(unsigned long long), e->stream));
-    GWB200_CUDA_TRY(e->timer.record_start(e->stream));
-    if (const int rc = extension_launch(e, query, qlen, target, tlen, score_threshold, seeds, n, e->kept_d.p, e->num_kept_d.p, e->examined_d.p))
-        return rc;
-    if (const int rc = sort_unique(e, qlen, tlen, e->kept_d.p, e->num_kept_d.p, n, out, num_out))
-        return rc;
-    GWB200_CUDA_TRY(e->timer.record_stop(e->stream));
-    e->launched = true;
-    return GWB200_EXT_SUCCESS;
-}
-
 } // namespace
 
 namespace gwb200
@@ -116,16 +108,19 @@ namespace extender
 {
 
 // Step 1 of an extend call: extends seeds [0, n) and appends the segments it keeps to kept[*num_kept ...] (one atomic per kept
-// segment), adding the positions it examines to *examined. Nothing is cleared, so successive calls append to one buffer.
+// segment), adding the positions it examines to *examined. Nothing is cleared, so successive calls append to one buffer. With
+// recs, target and query are record groups and every extension stays inside its seed's two records.
 int extension_launch(const gwb200_extender* e, const int8_t* query, int32_t qlen, const int8_t* target, int32_t tlen, int32_t score_threshold,
-                     const void* seeds, int32_t n, void* kept, int32_t* num_kept, unsigned long long* examined)
+                     const void* seeds, int32_t n, void* kept, int32_t* num_kept, unsigned long long* examined, const GroupRecords* recs)
 {
     if (n == 0)
         return 0;
-    const int32_t grid = static_cast<int32_t>(std::min<int64_t>(e->grid_max, (static_cast<int64_t>(n) + kWarpsPerCta - 1) / kWarpsPerCta));
-    auto kernel        = e->wide ? ungapped_xdrop_kernel<int64_t> : ungapped_xdrop_kernel<int32_t>;
+    const int32_t grid = static_cast<int32_t>(
+        std::min<int64_t>(recs ? e->grid_max_groups : e->grid_max, (static_cast<int64_t>(n) + kWarpsPerCta - 1) / kWarpsPerCta));
+    auto kernel = recs ? extension_kernel<true>(e->wide) : extension_kernel<false>(e->wide);
     kernel<<<grid, kWarpsPerCta * 32, 0, e->stream>>>(target, tlen, query, qlen, e->sub_d.p, e->no_entropy, e->xdrop, score_threshold,
-                                                      static_cast<const SeedPairD*>(seeds), n, static_cast<SspD*>(kept), num_kept, examined);
+                                                      static_cast<const SeedPairD*>(seeds), n, static_cast<SspD*>(kept), num_kept, examined,
+                                                      recs ? *recs : GroupRecords{});
     GWB200_CUDA_TRY(cudaGetLastError());
     count_launch(1);
     return 0;
@@ -169,8 +164,92 @@ int sort_unique(gwb200_extender* e, int32_t qlen, int32_t tlen, const void* kept
     return 0;
 }
 
+int sort_unique_groups(gwb200_extender* e, const GroupRecords& recs, int32_t tmax, int32_t qmax, const void* kept_v, const int32_t* num_kept,
+                       int32_t n, void* out_v, uint64_t* pair_out, int32_t* num_out)
+{
+    if (n == 0)
+    {
+        GWB200_CUDA_TRY(cudaMemsetAsync(num_out, 0, sizeof(int32_t), e->stream));
+        return 0;
+    }
+    size_t pair_select_bytes = 0;
+    GWB200_CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, pair_select_bytes, static_cast<uint64_t*>(nullptr), static_cast<uint8_t*>(nullptr),
+                                               static_cast<uint64_t*>(nullptr), static_cast<int32_t*>(nullptr), n, e->stream));
+    if (const int rc = ensure_sort(e, n))
+        return rc;
+    if (!e->local_d.ensure(n) || !e->pair_d.ensure(n) || !e->sorted_pair_d.ensure(n) || !e->cub_d.ensure(static_cast<int64_t>(pair_select_bytes)))
+        return bad_alloc();
+    size_t cub_bytes    = static_cast<size_t>(e->cub_d.n);
+    const int32_t sgrid = grid_for(n, e->n_sms, 256);
+    // pass 1: length descending, then score descending
+    group_local_kernel<<<sgrid, 256, 0, e->stream>>>(static_cast<const SspD*>(kept_v), n, recs, tmax, e->local_d.p, e->pair_d.p, e->keys_a.p,
+                                                     e->idx_a.p);
+    GWB200_CUDA_TRY(cudaGetLastError());
+    cub::DoubleBuffer<uint64_t> keys(e->keys_a.p, e->keys_b.p);
+    cub::DoubleBuffer<uint32_t> idx(e->idx_a.p, e->idx_b.p);
+    GWB200_CUDA_TRY(cub::DeviceRadixSort::SortPairs(e->cub_d.p, cub_bytes, keys, idx, n, 0, 32 + bits_for(static_cast<int64_t>(tmax) + 1),
+                                                    e->stream));
+    // pass 2 (stable): each record pair's diagonal rank and target, over the group's longest records
+    const int tbits = bits_for(tmax);
+    const int dbits = bits_for(static_cast<int64_t>(tmax) + qmax);
+    primary_keys_kernel<<<sgrid, 256, 0, e->stream>>>(e->local_d.p, num_kept, n, tmax, qmax, tbits, ~0ull, idx.Current(), keys.Current());
+    GWB200_CUDA_TRY(cudaGetLastError());
+    GWB200_CUDA_TRY(cub::DeviceRadixSort::SortPairs(e->cub_d.p, cub_bytes, keys, idx, n, 0, tbits + dbits, e->stream));
+    int launches = 7;
+    // pass 3 (stable): the record pair
+    const int64_t pairs = static_cast<int64_t>(recs.nt) * recs.nq;
+    if (pairs > 1)
+    {
+        pair_keys_kernel<<<sgrid, 256, 0, e->stream>>>(e->pair_d.p, n, idx.Current(), keys.Current());
+        GWB200_CUDA_TRY(cudaGetLastError());
+        GWB200_CUDA_TRY(cub::DeviceRadixSort::SortPairs(e->cub_d.p, cub_bytes, keys, idx, n, 0, bits_for(pairs - 1), e->stream));
+        launches += 2;
+    }
+    group_unique_flags_kernel<<<sgrid, 256, 0, e->stream>>>(e->local_d.p, e->pair_d.p, n, idx.Current(), e->sorted_d.p, e->sorted_pair_d.p,
+                                                            e->flags_d.p);
+    GWB200_CUDA_TRY(cudaGetLastError());
+    GWB200_CUDA_TRY(cub::DeviceSelect::Flagged(e->cub_d.p, cub_bytes, e->sorted_d.p, e->flags_d.p, static_cast<SspD*>(out_v), num_out, n,
+                                               e->stream));
+    GWB200_CUDA_TRY(cub::DeviceSelect::Flagged(e->cub_d.p, cub_bytes, e->sorted_pair_d.p, e->flags_d.p, pair_out, num_out, n, e->stream));
+    count_launch(launches);
+    return 0;
+}
+
 } // namespace extender
 } // namespace gwb200
+
+namespace
+{
+
+// The device path of both extend calls; pointers and sizes are already checked.
+int run_extend(gwb200_extender* e, const int8_t* query, int32_t qlen, const int8_t* target, int32_t tlen, int32_t score_threshold,
+               const SeedPairD* seeds, int32_t n, SspD* out, int32_t* num_out)
+{
+    DeviceGuard guard(e->device_id);
+    e->launched = false;
+    if (n == 0)
+    {
+        GWB200_CUDA_TRY(cudaMemsetAsync(num_out, 0, sizeof(int32_t), e->stream));
+        return GWB200_EXT_SUCCESS;
+    }
+    if (!e->kept_d.ensure(n) || !e->num_kept_d.ensure(1) || !e->examined_d.ensure(1))
+        return bad_alloc();
+    if (const int rc = ensure_sort(e, n))
+        return rc;
+    GWB200_CUDA_TRY(cudaMemsetAsync(e->num_kept_d.p, 0, sizeof(int32_t), e->stream));
+    GWB200_CUDA_TRY(cudaMemsetAsync(e->examined_d.p, 0, sizeof(unsigned long long), e->stream));
+    GWB200_CUDA_TRY(e->timer.record_start(e->stream));
+    if (const int rc =
+            extension_launch(e, query, qlen, target, tlen, score_threshold, seeds, n, e->kept_d.p, e->num_kept_d.p, e->examined_d.p, nullptr))
+        return rc;
+    if (const int rc = sort_unique(e, qlen, tlen, e->kept_d.p, e->num_kept_d.p, n, out, num_out))
+        return rc;
+    GWB200_CUDA_TRY(e->timer.record_stop(e->stream));
+    e->launched = true;
+    return GWB200_EXT_SUCCESS;
+}
+
+} // namespace
 
 extern "C" {
 
@@ -202,11 +281,9 @@ int gwb200_extender_create_with_allocator(gwb200_extender** out, const int32_t* 
     e->no_entropy      = no_entropy ? 1 : 0;
     e->wide            = !narrow_scores_suffice(score_mat, xdrop_threshold);
     e->hooks           = MemHooks(alloc_fn, free_fn, user);
-    int per_sm = 0;
     cudaDeviceGetAttribute(&e->n_sms, cudaDevAttrMultiProcessorCount, device_id);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, e->wide ? ungapped_xdrop_kernel<int64_t> : ungapped_xdrop_kernel<int32_t>,
-                                                  kWarpsPerCta * 32, 0);
-    e->grid_max = std::max(1, e->n_sms * per_sm);
+    e->grid_max        = resident_ctas(reinterpret_cast<const void*>(extension_kernel<false>(e->wide)), e->n_sms);
+    e->grid_max_groups = resident_ctas(reinterpret_cast<const void*>(extension_kernel<true>(e->wide)), e->n_sms);
     if (!e->sub_d.ensure(kNuc * kNuc))
     {
         gwb200_extender_destroy(e);

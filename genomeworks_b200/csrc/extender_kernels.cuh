@@ -11,6 +11,8 @@
 #include <climits>
 #include <cuda_runtime.h>
 
+#include "extender_internal.cuh"
+
 namespace gwb200
 {
 namespace extender
@@ -207,12 +209,13 @@ __device__ __forceinline__ ExtResult extend_one_side(const int8_t* __restrict__ 
 
 // Extends every seed; a kept segment is appended to `kept` at an index taken from `*num_kept`. Seeds that do not lie inside
 // both sequences produce nothing. `examined` accumulates the positions the extensions covered. ScoreT: see
-// narrow_scores_suffice.
-template <typename ScoreT>
+// narrow_scores_suffice. kBounded: target and query are record groups (`recs`); each extension stops at the ends of its
+// seed's two records, never past them, whatever the codes beyond score.
+template <typename ScoreT, bool kBounded>
 __global__ void __launch_bounds__(kWarpsPerCta * 32) ungapped_xdrop_kernel(
     const int8_t* __restrict__ target, int32_t tlen, const int8_t* __restrict__ query, int32_t qlen, const int32_t* __restrict__ sub_mat,
     int32_t no_entropy, int32_t xdrop, int32_t score_threshold, const SeedPairD* __restrict__ seeds, int32_t n, SspD* __restrict__ kept,
-    int32_t* __restrict__ num_kept, unsigned long long* __restrict__ examined_total)
+    int32_t* __restrict__ num_kept, unsigned long long* __restrict__ examined_total, GroupRecords recs)
 {
     __shared__ int32_t sub[kNuc * kNuc];
     for (int i = threadIdx.x; i < kNuc * kNuc; i += blockDim.x)
@@ -228,9 +231,19 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) ungapped_xdrop_kernel(
         const int64_t ts = sp.target, qs = sp.query;
         if (ts >= tlen || qs >= qlen)
             continue;
+        int64_t t_begin = 0, t_end = tlen, q_begin = 0, q_end = qlen;
+        if constexpr (kBounded)
+        {
+            const int32_t tk = record_of(recs.t_start, recs.nt, sp.target), qk = record_of(recs.q_start, recs.nq, sp.query);
+            t_begin          = __ldg(recs.t_start + tk);
+            t_end            = __ldg(recs.t_end + tk);
+            q_begin          = __ldg(recs.q_start + qk);
+            q_end            = __ldg(recs.q_end + qk);
+        }
         const ExtResult r =
-            extend_one_side<false, ScoreT>(target, tlen, query, qlen, ts, qs, min(tlen - ts, qlen - qs), sub, xdrop, examined);
-        const ExtResult l = extend_one_side<true, ScoreT>(target, tlen, query, qlen, ts, qs, min(ts, qs), sub, xdrop, examined);
+            extend_one_side<false, ScoreT>(target, tlen, query, qlen, ts, qs, min(t_end - ts, q_end - qs), sub, xdrop, examined);
+        const ExtResult l =
+            extend_one_side<true, ScoreT>(target, tlen, query, qlen, ts, qs, min(ts - t_begin, qs - q_begin), sub, xdrop, examined);
         const int64_t total  = r.max_score + l.max_score; // >= 0
         const int32_t length = r.max_pos + l.max_pos;
         int64_t score        = total;
@@ -343,6 +356,48 @@ __global__ void unique_flags_kernel(const SspD* __restrict__ kept, const int32_t
         {
             flags[i] = 0;
         }
+    }
+}
+
+// The n segments of a group pair, kept in group coordinates: each in its records' own coordinates, its record pair
+// (target record * recs.nq + query record), and the key of the first sort pass over the group's longest target record
+// (DESIGN.md section 21.3).
+__global__ void group_local_kernel(const SspD* __restrict__ kept, int32_t n, GroupRecords recs, int32_t tmax, SspD* __restrict__ local,
+                                   uint64_t* __restrict__ pair, uint64_t* __restrict__ keys, uint32_t* __restrict__ idx)
+{
+    for (int32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    {
+        SspD s           = kept[i];
+        const int32_t tk = record_of(recs.t_start, recs.nt, s.target), qk = record_of(recs.q_start, recs.nq, s.query);
+        s.target -= __ldg(recs.t_start + tk);
+        s.query -= __ldg(recs.q_start + qk);
+        local[i] = s;
+        pair[i]  = static_cast<uint64_t>(tk) * static_cast<uint64_t>(recs.nq) + static_cast<uint64_t>(qk);
+        keys[i]  = secondary_key(s, tmax);
+        idx[i]   = static_cast<uint32_t>(i);
+    }
+}
+
+// keys[i] = pair[idx[i]]: the last, most significant sort pass.
+__global__ void pair_keys_kernel(const uint64_t* __restrict__ pair, int32_t n, const uint32_t* __restrict__ idx, uint64_t* __restrict__ keys)
+{
+    for (int32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        keys[i] = pair[idx[i]];
+}
+
+// unique_flags_kernel over the sorted segments of a group pair, where a segment can only be contained in a predecessor of
+// the same record pair.
+__global__ void group_unique_flags_kernel(const SspD* __restrict__ local, const uint64_t* __restrict__ pair, int32_t n,
+                                          const uint32_t* __restrict__ idx, SspD* __restrict__ sorted, uint64_t* __restrict__ sorted_pair,
+                                          uint8_t* __restrict__ flags)
+{
+    for (int32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    {
+        const uint32_t k = idx[i];
+        const SspD cur   = local[k];
+        sorted[i]        = cur;
+        sorted_pair[i]   = pair[k];
+        flags[i] = (i == 0 || pair[k] != pair[idx[i - 1]] || !diagonal_overlap(cur, local[idx[i - 1]])) ? 1 : 0;
     }
 }
 

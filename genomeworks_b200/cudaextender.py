@@ -534,6 +534,17 @@ GENOME_DTYPE = np.dtype([("score", np.int64), ("target_record", np.int32), ("que
                          ("target_end", np.uint32), ("matches", np.int64), ("block_length", np.int64)])
 STRANDS = {"plus": 1, "minus": 2, "both": 3}
 STAGES = ("index", "count", "write", "ungapped", "gapped_pass1", "gapped_pass2")
+GROUP_STATS = ("target_groups", "query_groups", "gapped_pairs")
+DEFAULT_GROUP_BASES = 1 << 28
+
+
+def _group_bases(group_bases):
+    """Checks group_bases (DESIGN.md section 21) before any device work; -> int."""
+    if isinstance(group_bases, (bool, np.bool_)) or not isinstance(group_bases, (int, np.integer)):
+        raise TypeError("group_bases must be an integer")
+    if not 1 <= int(group_bases) < (1 << 31):
+        raise ValueError("group_bases must lie in [1, 2^31 - 1]")
+    return int(group_bases)
 
 
 def default_genome_params():
@@ -558,11 +569,14 @@ class GenomeAligner:
     """The aligner with fixed parameters; run(targets, queries) aligns every query record against every target record."""
 
     def __init__(self, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, round_anchors=0, chain=None,
-                 min_chain_score=None, **params):
+                 min_chain_score=None, group_bases=DEFAULT_GROUP_BASES, **params):
+        """group_bases: the most codes of one side's records the aligner seeds and extends together (DESIGN.md section 21). It
+        bounds the seeding stage's device memory and never changes the output; 1 runs every record on its own."""
         from ._lib import GenomeAlignerParams
         if strand not in STRANDS:
             raise ValueError("strand must be one of %s" % ", ".join(STRANDS))
         skip = _skip_args(skip_covered, round_anchors)
+        group_bases = _group_bases(group_bases)
         penalties, min_score = _chain_args(chain, min_chain_score)
         p = default_genome_params()
         unknown = set(params) - set(p)
@@ -586,6 +600,7 @@ class GenomeAligner:
         if rc == invalid_input:
             raise ValueError("invalid genome aligner parameters")
         check(rc)
+        check(lib().gwb200_genome_aligner_set_group_bases(self._h, C.c_int64(group_bases)))
         if skip[0]:
             check(lib().gwb200_genome_aligner_set_skip_covered(self._h, C.c_int32(skip[0]), C.c_int32(skip[1])))
         if penalties is not None:
@@ -618,7 +633,9 @@ class GenomeAligner:
         return out, [raw[offsets[k]:offsets[k + 1]] for k in range(n)]
 
     def last_stats(self):
-        """Of the last run: {stage: device ms} summed over every pair and strand, and the seeds, unique segments and alignments."""
+        """Of the last run: {stage: device ms} and the seeds, unique segments and alignments. Index, count, write and ungapped
+        ms are summed over every pair of record groups and strand (index over target groups), the gapped passes over every
+        record pair and strand."""
         ms = np.zeros(len(STAGES), dtype=np.float32)
         counts = np.zeros(3, dtype=np.int64)
         check(lib().gwb200_genome_aligner_last_stats(self._h, ms.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p)))
@@ -645,6 +662,13 @@ class GenomeAligner:
         check(lib().gwb200_genome_aligner_last_chain_count(self._h, C.byref(n)))
         return n.value
 
+    def last_group_stats(self):
+        """Of the last run: {target_groups, query_groups, gapped_pairs}, the last being the (record pair, strand)s that had SSPs
+        and went to the gapped stage (DESIGN.md section 21)."""
+        out = np.zeros(len(GROUP_STATS), dtype=np.int64)
+        check(lib().gwb200_genome_aligner_last_group_stats(self._h, out.ctypes.data_as(C.c_void_p)))
+        return dict(zip(GROUP_STATS, (int(v) for v in out)))
+
     def close(self):
         if self._h:
             lib().gwb200_genome_aligner_destroy(self._h)
@@ -658,7 +682,7 @@ class GenomeAligner:
 
 
 def align_genomes(targets, queries, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, chain=None,
-                  min_chain_score=None, **params):
+                  min_chain_score=None, group_bases=DEFAULT_GROUP_BASES, **params):
     """Aligns every query record against every target record on the plus strand, the minus strand or both. targets and queries
     are lists of sequences (str or int8 codes). Keyword parameters override gwb200_genome_aligner_default_params: score_matrix,
     xdrop, ssp_threshold, gap_open, gap_extend, ydrop, gapped_threshold, transition, block_size, traceback_budget. Returns
@@ -666,8 +690,10 @@ def align_genomes(targets, queries, strand="both", stream=None, device_id=0, all
     target forward. Bad parameters raise ValueError before any device work. skip_covered=True does not extend the anchors that
     lie on an alignment kept earlier for the same pair and strand (DESIGN.md section 18). chain=True or (D, A) extends only the
     SSPs of the highest-scoring colinear chain of each pair and strand (DESIGN.md section 19); with min_chain_score=S as well,
-    those of every chain scoring >= S (DESIGN.md section 20)."""
-    al = GenomeAligner(strand, stream, device_id, allocator, skip_covered, chain=chain, min_chain_score=min_chain_score, **params)
+    those of every chain scoring >= S (DESIGN.md section 20). group_bases (1 to 2^31 - 1) is the most codes of one side's
+    records seeded and extended together (DESIGN.md section 21); it bounds device memory and never changes the output."""
+    al = GenomeAligner(strand, stream, device_id, allocator, skip_covered, chain=chain, min_chain_score=min_chain_score,
+                       group_bases=group_bases, **params)
     try:
         return al.run(targets, queries)
     finally:

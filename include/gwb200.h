@@ -609,8 +609,9 @@ int32_t gwb200_genome_aligner_num_results(const gwb200_genome_aligner* aligner);
 int gwb200_genome_aligner_get_results(const gwb200_genome_aligner* aligner, gwb200_genome_alignment* out, int32_t capacity);
 int64_t gwb200_genome_aligner_cigar_bytes(const gwb200_genome_aligner* aligner);
 int gwb200_genome_aligner_get_cigars(const gwb200_genome_aligner* aligner, char* text, int64_t text_capacity, int64_t* offsets);
-/* Of the last run, summed over every pair and strand: device ms of index, count, write, ungapped, gapped pass 1 and gapped
- * pass 2 (stage_ms[6]), and the seeds, the unique segments and the alignments (counts[3]). */
+/* Of the last run: device ms of index, count, write and ungapped summed over every group pair and strand (index over target
+ * groups), of gapped pass 1 and gapped pass 2 summed over every record pair and strand (stage_ms[6]); and the seeds, the
+ * unique segments and the alignments (counts[3]). */
 int gwb200_genome_aligner_last_stats(const gwb200_genome_aligner* aligner, float* stage_ms, int64_t* counts);
 /* Puts the aligner's gapped extender in skip-covered mode (gwb200_gapped_extender_set_skip_covered) for later runs. Coverage
  * never crosses a (pair, strand), and minus-strand anchors are tested in the strand's own coordinates. */
@@ -640,6 +641,16 @@ int gwb200_genome_aligner_set_chain_min_score(gwb200_genome_aligner* aligner, in
 /* The number of chains the last run reported, summed over every pair and strand (one per chained (pair, strand) with the best
  * chain; zero with chaining off). */
 int gwb200_genome_aligner_last_chain_count(const gwb200_genome_aligner* aligner, int64_t* chains);
+/* Record groups (DESIGN.md section 21): each side's records are packed in order into groups whose 16-byte-aligned record slots
+ * (a record's length + 1, rounded up to 16) total at most group_bases codes; a record whose slot alone is larger forms its own
+ * group. Each target group is indexed once, and seeds and ungapped extension run once per (target group, query group,
+ * strand); the gapped stage runs per (record pair, strand) with SSPs. The output never depends on group_bases; it bounds the
+ * device memory of the seeding stage (about 18 bytes per target group code and 22 per query group code). Default 2^28; with
+ * 1 every record forms its own group. It holds for later runs. invalid_input for group_bases outside [1, 2^31 - 1], before
+ * the handle is looked at. */
+int gwb200_genome_aligner_set_group_bases(gwb200_genome_aligner* aligner, int64_t group_bases);
+/* Of the last run: target groups, query groups, and the (record pair, strand)s handed to the gapped stage (out[3]). */
+int gwb200_genome_aligner_last_group_stats(const gwb200_genome_aligner* aligner, int64_t* out);
 
 /* ------------------------------------------------------------------------------------------------
  * cudamapper (minimizer index)

@@ -1,20 +1,28 @@
 """Genome aligner benchmark: one JSON line per workload, with the aligner's defaults (both strands, transitions, the sample
 matrix, LASTZ-style gapped parameters, blocks of 2^25 seeds).
 
-    python tools/bench_genome_aligner.py [--steps K] [--warmup W] [--workloads sample,assembly]
+    python tools/bench_genome_aligner.py [--steps K] [--warmup W] [--workloads sample,assembly,contigs]
                                          [--modes default,skip,chain,chain+skip,chains,chains+skip] [--skip-covered]
-                                         [--min-chain-score 30000]
+                                         [--min-chain-score 30000] [--group-bases N] [--contigs 2000]
 
 Workloads:
   sample    the golden sample (one 250 kb record) against itself;
   assembly  a 10 Mb random target against a query assembled from 5-50 kb pieces of it, each diverged by 2-10 % (80 %
             substitutions, 10 % each 1-3 base insertions and deletions), about a third of them reverse-complemented, in a
             shuffled order. Every homologous gapped side ends within its piece.
+  contigs   the assembly workload's target cut at random points into --contigs records (a draft assembly). First against
+            the 80 pieces as separate query records, run grouped (--group-bases) and with every record on its own
+            (group_bases=1), alternating in one process, with identical outputs asserted; then grouped alone against the
+            query cut into --contigs records as well. The per-record run pays an index build per target record and the
+            launches and host synchronisations of every (target record, query record, strand), which is what grouping
+            (DESIGN.md section 21) removes; that is why this workload is many short records on both sides.
 
 Each line: the per-stage device ms of the last run (CUDA events summed over pairs and strands: index, count, write, ungapped,
 gapped pass 1 and pass 2), the seeds, unique segments and alignments, seeds/s of the seeding stage (count + write) and of the
 write pass alone with its bytes/s (8 bytes written per seed), and the wall time of a whole run (host clock, mean of `steps` runs
-after `warmup`). The card name and power limit are read in the same run. Writes nothing to the tree.
+after `warmup`). The card name and power limit are read in the same run. Writes nothing to the tree. Every line reports
+the group size and the aligner's group stats (target groups, query groups, record pairs and strands given to the gapped
+stage).
 
 --modes default,skip runs each workload in both modes in the same process, the runs alternating between them, and prints one
 line per mode; skip is the skip-covered mode (DESIGN.md section 18). A skip line adds the skip stats of the gapped stage and
@@ -90,10 +98,42 @@ def key(r):
                                      "target_end"))
 
 
-def run(name, targets, queries, steps, warmup, extra, modes=("default",), min_chain_score=30000, placed=None):
+def cut(seq, n, rng):
+    """seq cut at n - 1 distinct random points into n records."""
+    points = np.sort(rng.choice(np.arange(1, len(seq)), n - 1, replace=False))
+    return [seq[a:b] for a, b in zip(np.r_[0, points], np.r_[points, len(seq)])]
+
+
+def run_group_sizes(name, targets, queries, steps, warmup, extra, sizes):
+    """Default mode at each group size in `sizes`, the runs alternating; asserts that every size gives the first's output."""
+    from genomeworks_b200 import cudaextender as ce
+    aligners = {g: ce.GenomeAligner(group_bases=g) for g in sizes}
+    for _ in range(warmup):
+        for al in aligners.values():
+            al.run(targets, queries)
+    wall = dict.fromkeys(sizes, 0.0)
+    out = {}
+    for _ in range(steps):
+        for g, al in aligners.items():
+            t0 = time.perf_counter()
+            out[g] = al.run(targets, queries)
+            wall[g] += (time.perf_counter() - t0) / steps
+    first = out[sizes[0]]
+    for g, al in aligners.items():
+        same = bool(np.array_equal(out[g][0], first[0]) and out[g][1] == first[1])
+        assert same, "group_bases %d changed the output" % g
+        ms, counts = al.last_stats()
+        more = dict(extra, mode="default", group_bases=g, group_stats=al.last_group_stats(), target_records=len(targets),
+                    query_records=len(queries), same_output_as_group_bases=sizes[0] if len(sizes) > 1 else None)
+        al.close()
+        line(name, targets, queries, steps, warmup, out[g][0], wall[g], ms, counts, more)
+
+
+def run(name, targets, queries, steps, warmup, extra, modes=("default",), min_chain_score=30000, placed=None, group_bases=1 << 28):
     from genomeworks_b200 import cudaextender as ce
     aligners = {m: ce.GenomeAligner(skip_covered=m.endswith("skip"), chain=m.startswith("chain"),
-                                    min_chain_score=min_chain_score if m.startswith("chains") else None) for m in modes}
+                                    min_chain_score=min_chain_score if m.startswith("chains") else None, group_bases=group_bases)
+                for m in modes}
     for _ in range(warmup):
         for al in aligners.values():
             al.run(targets, queries)
@@ -106,7 +146,7 @@ def run(name, targets, queries, steps, warmup, extra, modes=("default",), min_ch
             wall[m] += (time.perf_counter() - t0) / steps
     for m, al in aligners.items():
         ms, counts = al.last_stats()
-        more = dict(extra, mode=m)
+        more = dict(extra, mode=m, group_bases=group_bases, group_stats=al.last_group_stats())
         if m.startswith("chain"):
             more["chain_stats"] = al.last_chain_stats()
             more["chains"] = al.last_chain_count()
@@ -146,6 +186,8 @@ def main():
     ap.add_argument("--modes", default="default")
     ap.add_argument("--skip-covered", action="store_true")
     ap.add_argument("--min-chain-score", type=int, default=30000)
+    ap.add_argument("--group-bases", type=int, default=1 << 28)
+    ap.add_argument("--contigs", type=int, default=2000)
     a = ap.parse_args()
     modes = ["skip"] if a.skip_covered else a.modes.split(",")
     if set(modes) - {"default", "skip", "chain", "chain+skip", "chains", "chains+skip"}:
@@ -157,10 +199,17 @@ def main():
         if w == "sample":
             import extender_libs as xl
             seq, _, _ = xl.sample()
-            run("sample", [seq], [seq], a.steps, a.warmup, {}, modes, a.min_chain_score)
+            run("sample", [seq], [seq], a.steps, a.warmup, {}, modes, a.min_chain_score, group_bases=a.group_bases)
         elif w == "assembly":
             t, q, extra, placed = assembly()
-            run("assembly", t, q, a.steps, a.warmup, extra, modes, a.min_chain_score, placed)
+            run("assembly", t, q, a.steps, a.warmup, extra, modes, a.min_chain_score, placed, a.group_bases)
+        elif w == "contigs":
+            t, q, extra, placed = assembly()
+            rng = np.random.default_rng(7)
+            targets = cut(t[0], a.contigs, rng)
+            pieces = [q[0][qb:qe] for qb, qe, _, _, _ in placed]
+            run_group_sizes("contigs_x_pieces", targets, pieces, a.steps, a.warmup, extra, [a.group_bases, 1])
+            run_group_sizes("contigs_x_contigs", targets, cut(q[0], a.contigs, rng), a.steps, a.warmup, extra, [a.group_bases])
         else:
             sys.exit("unknown workload " + w)
 

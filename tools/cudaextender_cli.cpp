@@ -60,6 +60,10 @@ namespace
         --chain-min-score=S
             with --chain, extend the SSPs of every colinear chain scoring at least S (any 64-bit integer) instead of the
             best chain only
+        --group-bases=N
+            seed and extend the records of each file together in groups of at most N codes, each record in a slot of its
+            length + 1 rounded up to 16 [268435456]; bounds device memory, the output does not depend on it, and 1 aligns
+            every record on its own
         -h, --help
             this text
         -v, --version
@@ -147,7 +151,7 @@ int main(int argc, char* argv[])
         {"gap-extend", required_argument, 0, 'e'},      {"gapped-threshold", required_argument, 0, 'g'},
         {"block-size", required_argument, 0, 'B'},      {"traceback-budget", required_argument, 0, 'b'},
         {"skip-covered", no_argument, 0, 257},          {"chain", optional_argument, 0, 258},
-        {"chain-min-score", required_argument, 0, 259},
+        {"chain-min-score", required_argument, 0, 259}, {"group-bases", required_argument, 0, 260},
         {"version", no_argument, 0, 'v'},               {"help", no_argument, 0, 'h'},
         {0, 0, 0, 0},
     };
@@ -157,6 +161,7 @@ int main(int argc, char* argv[])
     bool skip_covered = false, chain = false, chain_all = false;
     int32_t chain_pen[2] = {0, 0};
     int64_t chain_min    = 0;
+    int64_t group_bases  = int64_t(1) << 28;
     int argument      = 0;
     while ((argument = getopt_long(argc, argv, "s:x:T:y:o:e:g:B:b:vh", options, nullptr)) != -1)
     {
@@ -200,6 +205,7 @@ int main(int argc, char* argv[])
             chain_all = true;
             chain_min = to_int(optarg, "chain-min-score", INT64_MIN, INT64_MAX);
             break;
+        case 260: group_bases = to_int(optarg, "group-bases", 1, i32); break;
         case 'x': p.xdrop = static_cast<int32_t>(to_int(optarg, "xdrop", 0, i32)); break;
         case 'T': p.ssp_threshold = static_cast<int32_t>(to_int(optarg, "ssp-threshold", -i32 - 1, i32)); break;
         case 'y': p.ydrop = static_cast<int32_t>(to_int(optarg, "ydrop", 0, 1 << 28)); break;
@@ -239,6 +245,8 @@ int main(int argc, char* argv[])
         fail("could not set chaining");
     if (chain_all && gwb200_genome_aligner_set_chain_min_score(a, 1, chain_min) != 0)
         fail("could not set the minimum chain score");
+    if (gwb200_genome_aligner_set_group_bases(a, group_bases) != 0)
+        fail("could not set the group size");
     const int rc = gwb200_genome_aligner_run(a, tcodes.data(), toff.data(), static_cast<int32_t>(targets.size()), qcodes.data(), qoff.data(),
                                              static_cast<int32_t>(queries.size()));
     if (rc != 0)
