@@ -282,6 +282,7 @@ def lib():
     L.gwb200_seeder_create_with_allocator.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                                       C.c_void_p]
     L.gwb200_seeder_destroy.argtypes = [C.c_void_p]
+    L.gwb200_seeder_set_seed.argtypes = [C.c_void_p, C.c_char_p, C.c_int64]
     L.gwb200_seeder_destroy.restype = None
     L.gwb200_seeder_index_target.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
     L.gwb200_seeder_count.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
@@ -324,6 +325,7 @@ def lib():
     L.gwb200_genome_aligner_last_chain_count.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     L.gwb200_genome_aligner_set_group_bases.argtypes = [C.c_void_p, C.c_int64]
     L.gwb200_genome_aligner_last_group_stats.argtypes = [C.c_void_p, C.c_void_p]
+    L.gwb200_genome_aligner_set_seed.argtypes = [C.c_void_p, C.c_char_p, C.c_int64]
     L.gwb200_index_create.argtypes = [C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int64, C.c_uint32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_double, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     L.gwb200_index_wait.argtypes = [C.c_void_p]

@@ -12,12 +12,14 @@
 // to forward coordinates and counts the PAF columns. In skip-covered mode (DESIGN.md section 18) the gapped extender of each pair and strand runs the
 // sequential rule in its own coordinates. With chaining on (DESIGN.md section 19) the unique segments of each pair and strand
 // are chained first, and only the chain's segments go to the gapped extender; with all chains on (DESIGN.md section 20), the
-// union of every chain scoring at least the minimum does.
+// union of every chain scoring at least the minimum does. With a word cap (DESIGN.md section 22), every target group is indexed
+// once before seeding to count its words into one table for the whole target side, which the seeder then caps by.
 
 #include "../../include/gwb200.h"
 #include "chain_internal.cuh"
 #include "common.cuh"
 #include "extender_internal.cuh"
+#include "seeder_internal.cuh"
 
 #include <cub/device/device_run_length_encode.cuh>
 
@@ -110,6 +112,9 @@ struct gwb200_genome_aligner
     bool chain_all       = false;  // every chain scoring >= chain_min instead of the best one
     int64_t chain_min    = 0;
     int64_t group_bases  = kDefaultGroupBases;
+    int64_t max_word_count = 0; // the word cap, 0 = off
+
+    DevBuf<unsigned long long> words_d{&hooks}; // with the cap on: every key's count over all target records, saturated at cap + 1
 
     DevBuf<int8_t> target_d{&hooks}, query_d{&hooks}; // the target group and the query group
     DevBuf<uint32_t> t_start_d{&hooks}, t_end_d{&hooks}, q_start_d{&hooks}, q_end_d{&hooks}; // their records' bounds
@@ -565,14 +570,38 @@ int run(gwb200_genome_aligner* a, const int8_t* targets, const int64_t* toff, in
     Side t{tl, targets, toff, a->t_staging, a->target_d, a->t_start_d, a->t_end_d};
     Side q{ql, queries, qoff, a->q_staging, a->query_d, a->q_start_d, a->q_end_d};
     GWB200_CUDA_TRY(cudaMemsetAsync(a->examined_d.p, 0, sizeof(unsigned long long), a->stream));
+    const auto index = [&](int32_t tg) -> int {
+        if (const int rc = stage_group(a, t, tg))
+            return rc;
+        return static_cast<int>(timed(a, kIndex, [&] { return int64_t(gwb200_seeder_index_target(a->seeder, t.dev.p, tl.length(tg))); }));
+    };
+    // the word counts of every target record, from each target group's index; a single group's index is then kept for seeding
+    const bool count_words = a->max_word_count > 0 && tl.groups() > 0;
+    seeder::use_word_counts(a->seeder, nullptr);
+    if (count_words)
+    {
+        const int64_t keys = seeder::num_keys(a->seeder);
+        if (!a->words_d.ensure(keys))
+            return bad_alloc();
+        GWB200_CUDA_TRY(cudaMemsetAsync(a->words_d.p, 0, sizeof(unsigned long long) * keys, a->stream));
+        for (int32_t tg = 0; tg < tl.groups(); ++tg)
+        {
+            if (const int rc = index(tg))
+                return rc;
+            if (const int64_t rc = timed(a, kIndex, [&] {
+                    return int64_t(seeder::accumulate_word_counts(a->seeder, a->words_d.p, static_cast<unsigned long long>(a->max_word_count) + 1));
+                }))
+                return static_cast<int>(rc);
+        }
+        seeder::use_word_counts(a->seeder, a->words_d.p);
+    }
     int32_t staged_q = -1; // the query group on the device
     bool minus       = false; // it holds the minus strand
     for (int32_t tg = 0; tg < tl.groups(); ++tg)
     {
-        if (const int rc = stage_group(a, t, tg))
-            return rc;
-        if (const int64_t rc = timed(a, kIndex, [&] { return int64_t(gwb200_seeder_index_target(a->seeder, t.dev.p, tl.length(tg))); }))
-            return static_cast<int>(rc);
+        if (!(count_words && tl.groups() == 1))
+            if (const int rc = index(tg))
+                return rc;
         for (int32_t qg = 0; qg < ql.groups(); ++qg)
         {
             if (qg != staged_q)
@@ -813,6 +842,21 @@ int gwb200_genome_aligner_set_group_bases(gwb200_genome_aligner* a, int64_t grou
     if (!a)
         return set_error(GWB200_E_INVALID_ARGUMENT, "null genome aligner");
     a->group_bases = group_bases;
+    return GWB200_EXT_SUCCESS;
+}
+
+int gwb200_genome_aligner_set_seed(gwb200_genome_aligner* a, const char* pattern, int64_t max_word_count)
+{
+    seeder::SeedPattern p{};
+    if (!seeder::parse_pattern(pattern, &p) || max_word_count < 0)
+        return GWB200_EXT_INVALID_INPUT;
+    if (!a)
+        return set_error(GWB200_E_INVALID_ARGUMENT, "null genome aligner");
+    DeviceGuard guard(a->device_id);
+    if (const int rc = gwb200_seeder_set_seed(a->seeder, pattern, max_word_count))
+        return rc;
+    a->max_word_count = max_word_count;
+    a->words_d.release();
     return GWB200_EXT_SUCCESS;
 }
 

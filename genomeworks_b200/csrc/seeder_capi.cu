@@ -1,8 +1,8 @@
-// gw-b200: host engine + C ABI of the spaced-seed seeder (include/gwb200.h, DESIGN.md section 17). Kernels: seeder_kernels.cuh.
-// No CPU fallback.
+// gw-b200: host engine + C ABI of the spaced-seed seeder (include/gwb200.h, DESIGN.md sections 17 and 22). Kernels:
+// seeder_kernels.cuh. No CPU fallback.
 //
-// index_target: keys of every target window -> one stable cub radix sort of (key, position) over 25 key bits -> the end of
-// every key's run (a scatter, then a max-scan over the 2^24 keys). count: keys of every query window -> per-position seed
+// index_target: keys of every target window -> one stable cub radix sort of (key, position) over 2W + 1 key bits -> the end of
+// every key's run (a scatter, then a max-scan over the 2^2W keys). count: keys of every query window -> per-position seed
 // counts -> an int64 exclusive scan, whose last entry is the total, read back. get_block: the output-driven write pass over
 // one block of the global order, enqueued without waiting.
 
@@ -14,6 +14,7 @@
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
+#include <string>
 
 using namespace gwb200;
 using namespace gwb200::seeder;
@@ -24,6 +25,9 @@ struct gwb200_seeder
     cudaStream_t stream = nullptr;
     int32_t transition = 1;
     int32_t n_sms      = 0;
+    SeedPattern pattern{};
+    int64_t cap                            = 0;       // the word cap, 0 = off
+    const unsigned long long* word_counts  = nullptr; // the caller's word counts (use_word_counts), or the runs' own lengths
     MemHooks hooks;
 
     DevBuf<int8_t> seq_d{&hooks}; // the sequence being keyed (target, then query)
@@ -62,6 +66,68 @@ int stage(gwb200_seeder* s, const int8_t* seq, int64_t len)
 
 } // namespace
 
+namespace gwb200
+{
+namespace seeder
+{
+
+bool parse_pattern(const char* text, SeedPattern* out)
+{
+    if (!text)
+        return false;
+    std::string bits = text;
+    if (bits == "12of19")
+        bits = "1110100110010101111";
+    else if (bits == "14of22")
+        bits = "1110101100110010101111";
+    else if (bits.compare(0, 5, "match") == 0)
+    {
+        const std::string n = bits.substr(5);
+        if (n.empty() || n.size() > 2 || n[0] < '1' || n[0] > '9' || (n.size() == 2 && (n[1] < '0' || n[1] > '9')))
+            return false;
+        const int w = std::stoi(n);
+        if (w > kMaxWeight)
+            return false;
+        bits.assign(static_cast<size_t>(w), '1');
+    }
+    if (bits.empty() || bits.size() > static_cast<size_t>(kMaxSpan) || bits.front() != '1' || bits.back() != '1')
+        return false;
+    SeedPattern p{};
+    p.span = static_cast<int32_t>(bits.size());
+    for (int i = 0; i < p.span; ++i)
+    {
+        if (bits[i] != '0' && bits[i] != '1')
+            return false;
+        if (bits[i] == '1')
+        {
+            if (p.weight == kMaxWeight)
+                return false;
+            p.care[p.weight++] = static_cast<int8_t>(i);
+        }
+    }
+    *out = p;
+    return true;
+}
+
+int64_t num_keys(const gwb200_seeder* s) { return s->pattern.keys(); }
+
+int accumulate_word_counts(gwb200_seeder* s, unsigned long long* counts, unsigned long long saturate)
+{
+    if (s->tlen < 0)
+        return set_error(GWB200_E_RUNTIME, "no target indexed: call index_target first");
+    DeviceGuard guard(s->device_id);
+    const int64_t keys = s->pattern.keys();
+    word_count_kernel<<<grid_for(keys, s->n_sms, 256), 256, 0, s->stream>>>(s->run_end_d.p, keys, saturate, counts);
+    GWB200_CUDA_TRY(cudaGetLastError());
+    count_launch(1);
+    return 0;
+}
+
+void use_word_counts(gwb200_seeder* s, const unsigned long long* counts) { s->word_counts = counts; }
+
+} // namespace seeder
+} // namespace gwb200
+
 extern "C" {
 
 int gwb200_seeder_create(gwb200_seeder** out, int32_t transition, void* stream, int32_t device_id)
@@ -82,6 +148,7 @@ int gwb200_seeder_create_with_allocator(gwb200_seeder** out, int32_t transition,
     s->device_id     = device_id;
     s->stream        = static_cast<cudaStream_t>(stream);
     s->transition    = transition ? 1 : 0;
+    parse_pattern("12of19", &s->pattern);
     s->hooks         = MemHooks(alloc_fn, free_fn, user);
     cudaDeviceGetAttribute(&s->n_sms, cudaDevAttrMultiProcessorCount, device_id);
     *out = s;
@@ -97,6 +164,25 @@ void gwb200_seeder_destroy(gwb200_seeder* s)
     delete s;
 }
 
+int gwb200_seeder_set_seed(gwb200_seeder* s, const char* pattern, int64_t max_word_count)
+{
+    SeedPattern p{};
+    if (!parse_pattern(pattern, &p) || max_word_count < 0)
+        return GWB200_EXT_INVALID_INPUT;
+    if (!s)
+        return set_error(GWB200_E_INVALID_ARGUMENT, "null seeder");
+    DeviceGuard guard(s->device_id);
+    GWB200_CUDA_TRY(cudaStreamSynchronize(s->stream)); // no pending block reads the tables
+    s->pattern = p;
+    s->cap     = max_word_count;
+    s->tlen = s->qlen = -1;
+    s->timed[0] = s->timed[1] = s->timed[2] = false;
+    // the run-end tables have 2^2W entries: a lighter pattern does not keep a heavier one's
+    s->ends_d.release();
+    s->run_end_d.release();
+    return GWB200_EXT_SUCCESS;
+}
+
 int gwb200_seeder_index_target(gwb200_seeder* s, const int8_t* target, int64_t target_length)
 {
     if (!length_ok(target, target_length))
@@ -107,34 +193,35 @@ int gwb200_seeder_index_target(gwb200_seeder* s, const int8_t* target, int64_t t
     s->tlen = s->qlen = -1;
     s->timed[0] = s->timed[1] = s->timed[2] = false;
     const int64_t n = target_length;
+    const int64_t n_keys = s->pattern.keys();
+    const int key_bits   = s->pattern.key_bits();
     cub::DoubleBuffer<uint32_t> keys(nullptr, nullptr), pos(nullptr, nullptr);
     size_t sort_bytes = 0, scan_bytes = 0;
-    GWB200_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys, pos, std::max<int64_t>(n, 1), 0, kKeyBits, s->stream));
+    GWB200_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys, pos, std::max<int64_t>(n, 1), 0, key_bits, s->stream));
     GWB200_CUDA_TRY(cub::DeviceScan::InclusiveScan(nullptr, scan_bytes, static_cast<int32_t*>(nullptr), static_cast<int32_t*>(nullptr), MaxOp(),
-                                                   static_cast<int64_t>(kKeys), s->stream));
+                                                   n_keys, s->stream));
     if (!s->keys_a.ensure(std::max<int64_t>(n, 1)) || !s->keys_b.ensure(std::max<int64_t>(n, 1)) || !s->pos_a.ensure(std::max<int64_t>(n, 1)) ||
-        !s->pos_b.ensure(std::max<int64_t>(n, 1)) || !s->ends_d.ensure(kKeys) || !s->run_end_d.ensure(kKeys) ||
+        !s->pos_b.ensure(std::max<int64_t>(n, 1)) || !s->ends_d.ensure(n_keys) || !s->run_end_d.ensure(n_keys) ||
         !s->cub_d.ensure(static_cast<int64_t>(std::max(sort_bytes, scan_bytes))))
         return bad_alloc();
     if (const int rc = stage(s, target, n))
         return rc;
     size_t cub_bytes = static_cast<size_t>(s->cub_d.n);
     GWB200_CUDA_TRY(s->t_index.record_start(s->stream));
-    GWB200_CUDA_TRY(cudaMemsetAsync(s->ends_d.p, 0, sizeof(int32_t) * kKeys, s->stream));
+    GWB200_CUDA_TRY(cudaMemsetAsync(s->ends_d.p, 0, sizeof(int32_t) * n_keys, s->stream));
     keys = cub::DoubleBuffer<uint32_t>(s->keys_a.p, s->keys_b.p);
     pos  = cub::DoubleBuffer<uint32_t>(s->pos_a.p, s->pos_b.p);
     if (n > 0)
     {
         const int grid = grid_for(n, s->n_sms, 256);
-        seed_keys_kernel<<<grid, 256, 0, s->stream>>>(s->seq_d.p, n, s->keys_a.p, s->pos_a.p);
+        seed_keys_kernel<<<grid, 256, 0, s->stream>>>(s->seq_d.p, n, s->pattern, s->keys_a.p, s->pos_a.p);
         GWB200_CUDA_TRY(cudaGetLastError());
-        GWB200_CUDA_TRY(cub::DeviceRadixSort::SortPairs(s->cub_d.p, cub_bytes, keys, pos, n, 0, kKeyBits, s->stream));
-        run_ends_kernel<<<grid, 256, 0, s->stream>>>(keys.Current(), n, s->ends_d.p);
+        GWB200_CUDA_TRY(cub::DeviceRadixSort::SortPairs(s->cub_d.p, cub_bytes, keys, pos, n, 0, key_bits, s->stream));
+        run_ends_kernel<<<grid, 256, 0, s->stream>>>(keys.Current(), n, s->pattern.keys(), s->ends_d.p);
         GWB200_CUDA_TRY(cudaGetLastError());
         count_launch(3);
     }
-    GWB200_CUDA_TRY(cub::DeviceScan::InclusiveScan(s->cub_d.p, cub_bytes, s->ends_d.p, s->run_end_d.p, MaxOp(), static_cast<int64_t>(kKeys),
-                                                   s->stream));
+    GWB200_CUDA_TRY(cub::DeviceScan::InclusiveScan(s->cub_d.p, cub_bytes, s->ends_d.p, s->run_end_d.p, MaxOp(), n_keys, s->stream));
     count_launch(1);
     GWB200_CUDA_TRY(s->t_index.record_stop(s->stream));
     s->sorted_pos = pos.Current();
@@ -170,9 +257,10 @@ int64_t gwb200_seeder_count(gwb200_seeder* s, const int8_t* query, int64_t query
     if (n > 0)
     {
         const int grid = grid_for(n, s->n_sms, 256);
-        seed_keys_kernel<<<grid, 256, 0, s->stream>>>(s->seq_d.p, n, s->qkeys_d.p, nullptr);
+        seed_keys_kernel<<<grid, 256, 0, s->stream>>>(s->seq_d.p, n, s->pattern, s->qkeys_d.p, nullptr);
         GWB200_CUDA_TRY(cudaGetLastError());
-        seed_count_kernel<<<grid, 256, 0, s->stream>>>(s->qkeys_d.p, n, s->run_end_d.p, s->transition, s->counts_d.p);
+        seed_count_kernel<<<grid, 256, 0, s->stream>>>(s->qkeys_d.p, n, s->pattern, s->run_end_d.p, s->word_counts, s->cap, s->transition,
+                                                       s->counts_d.p);
         GWB200_CUDA_TRY(cudaGetLastError());
         count_launch(2);
     }
@@ -200,8 +288,9 @@ int gwb200_seeder_get_block(gwb200_seeder* s, int64_t first, int64_t count, void
         return GWB200_EXT_SUCCESS;
     DeviceGuard guard(s->device_id);
     GWB200_CUDA_TRY(s->t_write.record_start(s->stream));
-    seed_write_kernel<<<grid_for(count, s->n_sms, 256), 256, 0, s->stream>>>(s->qkeys_d.p, s->offsets_d.p, s->qlen, s->run_end_d.p,
-                                                                             s->sorted_pos, first, count, static_cast<SeedPairD*>(d_out));
+    seed_write_kernel<<<grid_for(count, s->n_sms, 256), 256, 0, s->stream>>>(s->qkeys_d.p, s->offsets_d.p, s->qlen, s->pattern, s->run_end_d.p,
+                                                                             s->word_counts, s->cap, s->sorted_pos, first, count,
+                                                                             static_cast<SeedPairD*>(d_out));
     GWB200_CUDA_TRY(cudaGetLastError());
     GWB200_CUDA_TRY(s->t_write.record_stop(s->stream));
     count_launch(1);

@@ -14,6 +14,7 @@ over two sets of records.
 There is no CPU fallback: without a CUDA device create_extender and create_gapped_extender raise.
 """
 import ctypes as C
+import re
 
 import numpy as np
 
@@ -282,7 +283,38 @@ def create_gapped_extender(score_matrix, gap_open, gap_extend, ydrop, budget_byt
     return GappedXDrop(score_matrix, gap_open, gap_extend, ydrop, budget_bytes, stream, device_id, allocator, skip_covered, round_anchors)
 
 
-# Seeding (DESIGN.md section 17): the hits of LASTZ's 12-of-19 spaced seed, in the global order of include/gwb200.h.
+# Seeding (DESIGN.md sections 17 and 22): the hits of a spaced seed (LASTZ's 12-of-19 by default), in the global order of
+# include/gwb200.h.
+DEFAULT_SEED = "12of19"
+NAMED_SEEDS = {"12of19": "1110100110010101111", "14of22": "1110101100110010101111"}
+MAX_SEED_SPAN, MAX_SEED_WEIGHT = 32, 14
+
+
+def seed_pattern(seed):
+    """The 0/1 string of a seed pattern (DESIGN.md section 22.1): "12of19", "14of22", "match<N>" (N ones, 1 <= N <= 14) or a
+    string of 0 and 1 with a 1 at both ends, span 1 to 32 and 1 to 14 ones. TypeError for a non-string, ValueError otherwise."""
+    if not isinstance(seed, str):
+        raise TypeError("seed must be a string")
+    bits = NAMED_SEEDS.get(seed, seed)
+    m = re.fullmatch(r"match([1-9][0-9]?)", seed)
+    if m:
+        bits = "1" * int(m.group(1)) if int(m.group(1)) <= MAX_SEED_WEIGHT else ""
+    if (not re.fullmatch(r"1([01]*1)?", bits) or len(bits) > MAX_SEED_SPAN or bits.count("1") > MAX_SEED_WEIGHT):
+        raise ValueError("seed must be 12of19, 14of22, match<N> for N = 1 ... 14, or a string of 0 and 1 with a 1 at both ends, "
+                         "of span 1 to 32 with 1 to 14 ones; got %r" % seed)
+    return bits
+
+
+def _seed_args(seed, max_word_count):
+    """Checks a seed pattern and word cap before any device work; -> (seed bytes, cap)."""
+    seed_pattern(seed)
+    if isinstance(max_word_count, (bool, np.bool_)) or not isinstance(max_word_count, (int, np.integer)):
+        raise TypeError("max_word_count must be an integer")
+    if not 0 <= int(max_word_count) <= INT64_MAX:
+        raise ValueError("max_word_count must lie in [0, 2^63 - 1] (0 turns the word cap off)")
+    return seed.encode(), int(max_word_count)
+
+
 def _seq_arg(seq):
     """(pointer, length, object to keep alive) of a sequence: a torch tensor (host or CUDA) is passed by address; anything else
     is encoded / converted to int8 codes on the host."""
@@ -294,14 +326,23 @@ def _seq_arg(seq):
 
 class Seeder:
     """Spaced-seed seeder: index_target(target) once, then count(query) and get_block(first, count) for any number of queries.
-    Sequences are int8 codes (numpy, str, or torch tensors on the host or the device)."""
+    Sequences are int8 codes (numpy, str, or torch tensors on the host or the device). seed and max_word_count as set_seed."""
 
-    def __init__(self, transition=True, stream=None, device_id=0, allocator=None):
+    def __init__(self, transition=True, stream=None, device_id=0, allocator=None, seed=DEFAULT_SEED, max_word_count=0):
+        seed_args = _seed_args(seed, max_word_count)
         self._args = CallArgs(stream, allocator)
         self._device = device_id
         self._h = C.c_void_p()
         check(lib().gwb200_seeder_create_with_allocator(C.byref(self._h), C.c_int32(1 if transition else 0), self._args.stream,
                                                         C.c_int32(device_id), *self._args.mem))
+        if seed_args != (DEFAULT_SEED.encode(), 0):
+            check(lib().gwb200_seeder_set_seed(self._h, *seed_args))
+
+    def set_seed(self, seed=DEFAULT_SEED, max_word_count=0):
+        """The seed pattern (seed_pattern) and word cap of later calls (DESIGN.md section 22): with max_word_count N > 0, the
+        hits of a query word, exact or one transition variant, are dropped when the word occurs more than N times in the
+        target. Drops the target index: index_target again before count."""
+        check(lib().gwb200_seeder_set_seed(self._h, *_seed_args(seed, max_word_count)))
 
     def index_target(self, target):
         p, n, _ = _seq_arg(target)
@@ -362,9 +403,10 @@ class Seeder:
             pass
 
 
-def create_seeder(transition=True, stream=None, device_id=0, allocator=None):
-    """A Seeder; transition=False keeps only the exact hits. Without a CUDA device this raises RuntimeError."""
-    return Seeder(transition, stream, device_id, allocator)
+def create_seeder(transition=True, stream=None, device_id=0, allocator=None, seed=DEFAULT_SEED, max_word_count=0):
+    """A Seeder; transition=False keeps only the exact hits; seed and max_word_count as Seeder.set_seed. A bad seed or cap
+    raises TypeError or ValueError before any device work; without a CUDA device this raises RuntimeError."""
+    return Seeder(transition, stream, device_id, allocator, seed, max_word_count)
 
 
 # Chaining (DESIGN.md section 19): the highest-scoring colinear chain of scored segment pairs.
@@ -569,14 +611,17 @@ class GenomeAligner:
     """The aligner with fixed parameters; run(targets, queries) aligns every query record against every target record."""
 
     def __init__(self, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, round_anchors=0, chain=None,
-                 min_chain_score=None, group_bases=DEFAULT_GROUP_BASES, **params):
+                 min_chain_score=None, group_bases=DEFAULT_GROUP_BASES, seed=DEFAULT_SEED, max_word_count=0, **params):
         """group_bases: the most codes of one side's records the aligner seeds and extends together (DESIGN.md section 21). It
-        bounds the seeding stage's device memory and never changes the output; 1 runs every record on its own."""
+        bounds the seeding stage's device memory and never changes the output; 1 runs every record on its own. seed and
+        max_word_count: the seed pattern and word cap (Seeder.set_seed, DESIGN.md section 22); a word is counted over every
+        target record together."""
         from ._lib import GenomeAlignerParams
         if strand not in STRANDS:
             raise ValueError("strand must be one of %s" % ", ".join(STRANDS))
         skip = _skip_args(skip_covered, round_anchors)
         group_bases = _group_bases(group_bases)
+        seed_args = _seed_args(seed, max_word_count)
         penalties, min_score = _chain_args(chain, min_chain_score)
         p = default_genome_params()
         unknown = set(params) - set(p)
@@ -601,6 +646,8 @@ class GenomeAligner:
             raise ValueError("invalid genome aligner parameters")
         check(rc)
         check(lib().gwb200_genome_aligner_set_group_bases(self._h, C.c_int64(group_bases)))
+        if seed_args != (DEFAULT_SEED.encode(), 0):
+            check(lib().gwb200_genome_aligner_set_seed(self._h, *seed_args))
         if skip[0]:
             check(lib().gwb200_genome_aligner_set_skip_covered(self._h, C.c_int32(skip[0]), C.c_int32(skip[1])))
         if penalties is not None:
@@ -682,7 +729,7 @@ class GenomeAligner:
 
 
 def align_genomes(targets, queries, strand="both", stream=None, device_id=0, allocator=None, skip_covered=False, chain=None,
-                  min_chain_score=None, group_bases=DEFAULT_GROUP_BASES, **params):
+                  min_chain_score=None, group_bases=DEFAULT_GROUP_BASES, seed=DEFAULT_SEED, max_word_count=0, **params):
     """Aligns every query record against every target record on the plus strand, the minus strand or both. targets and queries
     are lists of sequences (str or int8 codes). Keyword parameters override gwb200_genome_aligner_default_params: score_matrix,
     xdrop, ssp_threshold, gap_open, gap_extend, ydrop, gapped_threshold, transition, block_size, traceback_budget. Returns
@@ -691,9 +738,11 @@ def align_genomes(targets, queries, strand="both", stream=None, device_id=0, all
     lie on an alignment kept earlier for the same pair and strand (DESIGN.md section 18). chain=True or (D, A) extends only the
     SSPs of the highest-scoring colinear chain of each pair and strand (DESIGN.md section 19); with min_chain_score=S as well,
     those of every chain scoring >= S (DESIGN.md section 20). group_bases (1 to 2^31 - 1) is the most codes of one side's
-    records seeded and extended together (DESIGN.md section 21); it bounds device memory and never changes the output."""
+    records seeded and extended together (DESIGN.md section 21); it bounds device memory and never changes the output. seed
+    ("12of19", "14of22", "match<N>" or a 0/1 pattern) and max_word_count N (0 = off) choose the seed and drop the hits of words
+    that occur more than N times over all target records (DESIGN.md section 22)."""
     al = GenomeAligner(strand, stream, device_id, allocator, skip_covered, chain=chain, min_chain_score=min_chain_score,
-                       group_bases=group_bases, **params)
+                       group_bases=group_bases, seed=seed, max_word_count=max_word_count, **params)
     try:
         return al.run(targets, queries)
     finally:

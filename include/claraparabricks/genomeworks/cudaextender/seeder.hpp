@@ -8,6 +8,7 @@
 
 #include <cstdint>
 #include <memory>
+#include <string>
 #include <stdexcept>
 
 namespace claraparabricks
@@ -17,9 +18,9 @@ namespace genomeworks
 namespace cudaextender
 {
 
-/// Hits of LASTZ's 12-of-19 spaced seed 1110100110010101111, exact or (with transitions) one transition apart, as SeedPair
-/// records in the global order of include/gwb200.h: query position ascending, then the exact bucket and the 12 transition
-/// buckets, then target position ascending.
+/// Hits of a spaced seed (LASTZ's 12-of-19 seed 1110100110010101111 unless set_seed changes it), exact or (with transitions)
+/// one transition apart, as SeedPair records in the global order of include/gwb200.h: query position ascending, then the exact
+/// bucket and the W transition buckets, then target position ascending.
 class Seeder
 {
 public:
@@ -33,6 +34,13 @@ public:
     ~Seeder() { gwb200_seeder_destroy(h_); }
     Seeder(const Seeder&) = delete;
     Seeder& operator=(const Seeder&) = delete;
+
+    /// The seed pattern ("12of19", "14of22", "match<N>" or a 0/1 string; gwb200_seeder_set_seed) and word cap (0 = off) of later
+    /// calls; drops the target index. invalid_input for a bad pattern or a negative cap.
+    StatusType set_seed(const std::string& pattern, int64_t max_word_count)
+    {
+        return static_cast<StatusType>(detail::check(gwb200_seeder_set_seed(h_, pattern.c_str(), max_word_count)));
+    }
 
     /// Indexes a target (host or device codes), kept for every later count(); invalid_input for 2^31 codes or more.
     StatusType index_target(const int8_t* target, int64_t target_length)

@@ -469,12 +469,16 @@ int gwb200_gapped_extender_set_skip_covered(gwb200_gapped_extender* extender, in
 int gwb200_gapped_extender_last_skip_stats(const gwb200_gapped_extender* extender, int64_t* out);
 
 /* ------------------------------------------------------------------------------------------------
- * cudaextender, seeding stage (DESIGN.md section 17): the hits of LASTZ's 12-of-19 spaced seed 1110100110010101111 between a
- * query and a target, as SeedPair records. The reference has no counterpart.
- * A seed is reported at the last position of its 19-position window; a window is used only when all 19 codes are in 0..3.
- * Two windows hit when their 12 care positions are equal or, with transitions on, differ by one transition (A <-> G or C <-> T,
- * code xor 2) at one care position. Global order: query position ascending; within one, the exact hits, then the transition
- * hits at care position 0, 1, ... 11; within each, target position ascending. A seed's rank in it is its global index.
+ * cudaextender, seeding stage (DESIGN.md sections 17 and 22): the hits of a spaced seed between a query and a target, as
+ * SeedPair records. The reference has no counterpart.
+ * The seed pattern is a string of care (1) and don't-care (0) positions with a 1 at both ends, span S (its length) 1 to 32 and
+ * weight W (its 1s) 1 to 14; the default is LASTZ's 12-of-19 seed 1110100110010101111 (set_seed changes it). A seed is reported
+ * at the last position of its S-position window; a window is used only when all S codes are in 0..3. Two windows hit when their
+ * W care positions are equal or, with transitions on, differ by one transition (A <-> G or C <-> T, code xor 2) at one care
+ * position. Global order: query position ascending; within one, the exact hits, then the transition hits at care position 0,
+ * 1, ... W - 1; within each, target position ascending. With a word cap N > 0, the hits of a query word (exact or one
+ * transition variant) are dropped when that word occurs more than N times in the target. A seed's rank in the order is its
+ * global index.
  * Sequences may be host or device pointers (copied with cudaMemcpyDefault); a length of 2^31 or more is invalid_input.
  * ---------------------------------------------------------------------------------------------- */
 
@@ -485,6 +489,11 @@ int gwb200_seeder_create(gwb200_seeder** out, int32_t transition, void* stream, 
 int gwb200_seeder_create_with_allocator(gwb200_seeder** out, int32_t transition, void* stream, int32_t device_id, gwb200_device_alloc_fn alloc_fn,
                                         gwb200_device_free_fn free_fn, void* user);
 void gwb200_seeder_destroy(gwb200_seeder* seeder);
+/* The seed pattern ("12of19", "14of22", "match<N>" for N ones, N = 1 ... 14, or a string of 0 and 1 as above) and the word cap
+ * (max_word_count; 0 turns it off) of later calls. Drops the target index: count reports no target indexed until the next
+ * index_target. The index needs two tables of 2^(2W) int32 (two 1 GiB tables at weight 14). invalid_input for any other pattern,
+ * NULL, or a negative cap, before the handle is looked at. */
+int gwb200_seeder_set_seed(gwb200_seeder* seeder, const char* pattern, int64_t max_word_count);
 /* Builds the target index (kept until the next index_target; the target itself is not). Enqueued without waiting. */
 int gwb200_seeder_index_target(gwb200_seeder* seeder, const int8_t* target, int64_t target_length);
 /* Counts the seeds of a query against the indexed target and returns their total (blocking). Every failure is a negative
@@ -651,6 +660,10 @@ int gwb200_genome_aligner_last_chain_count(const gwb200_genome_aligner* aligner,
 int gwb200_genome_aligner_set_group_bases(gwb200_genome_aligner* aligner, int64_t group_bases);
 /* Of the last run: target groups, query groups, and the (record pair, strand)s handed to the gapped stage (out[3]). */
 int gwb200_genome_aligner_last_group_stats(const gwb200_genome_aligner* aligner, int64_t* out);
+/* The seed pattern and word cap of later runs (gwb200_seeder_set_seed; default "12of19", no cap). With a cap N > 0, a word is
+ * counted over every target record together, on the forward strand, before any record is seeded, so the cap does not depend
+ * on group_bases or strand; that takes 2^(2W) more int64 of device memory. invalid_input as gwb200_seeder_set_seed. */
+int gwb200_genome_aligner_set_seed(gwb200_genome_aligner* aligner, const char* pattern, int64_t max_word_count);
 
 /* ------------------------------------------------------------------------------------------------
  * cudamapper (minimizer index)

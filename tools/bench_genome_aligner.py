@@ -1,9 +1,10 @@
 """Genome aligner benchmark: one JSON line per workload, with the aligner's defaults (both strands, transitions, the sample
 matrix, LASTZ-style gapped parameters, blocks of 2^25 seeds).
 
-    python tools/bench_genome_aligner.py [--steps K] [--warmup W] [--workloads sample,assembly,contigs]
+    python tools/bench_genome_aligner.py [--steps K] [--warmup W] [--workloads sample,assembly,contigs,repeats]
                                          [--modes default,skip,chain,chain+skip,chains,chains+skip] [--skip-covered]
                                          [--min-chain-score 30000] [--group-bases N] [--contigs 2000]
+                                         [--seed 12of19] [--max-word-count N] [--repeat-copies 300]
 
 Workloads:
   sample    the golden sample (one 250 kb record) against itself;
@@ -16,6 +17,12 @@ Workloads:
             query cut into --contigs records as well. The per-record run pays an index build per target record and the
             launches and host synchronisations of every (target record, query record, strand), which is what grouping
             (DESIGN.md section 21) removes; that is why this workload is many short records on both sides.
+  repeats   a repeat-rich pair that is not soft-masked: a 2 Mb random target and a 1 Mb random query, each carrying
+            --repeat-copies copies of one 300 bp element, every copy 5 % diverged from it. The seeds of the element grow with
+            the product of the copy counts, which is what the word cap (--max-word-count, DESIGN.md section 22) bounds.
+
+--seed (12of19, 14of22, match<N> or a 0/1 pattern) and --max-word-count (0 = no cap) set the seeding stage of every run
+(DESIGN.md section 22); every line reports them.
 
 Each line: the per-stage device ms of the last run (CUDA events summed over pairs and strands: index, count, write, ungapped,
 gapped pass 1 and pass 2), the seeds, unique segments and alignments, seeds/s of the seeding stage (count + write) and of the
@@ -104,10 +111,28 @@ def cut(seq, n, rng):
     return [seq[a:b] for a, b in zip(np.r_[0, points], np.r_[points, len(seq)])]
 
 
-def run_group_sizes(name, targets, queries, steps, warmup, extra, sizes):
+def repeats(copies, seed=2027, element=300, divergence=0.05):
+    """([target], [query], counts): 2 Mb and 1 Mb of random codes with `copies` diverged copies of one element inserted into
+    each at random points."""
+    import seeder_libs as sl
+    rng = np.random.default_rng(seed)
+    unit = rng.integers(0, 4, element).astype(np.int8)
+
+    def carrier(n):
+        base = rng.integers(0, 4, n).astype(np.int8)
+        points = np.sort(rng.choice(np.arange(1, n), copies, replace=False))
+        parts = [base[a:b] for a, b in zip(np.r_[0, points], np.r_[points, n])]
+        out = [parts[0]]
+        for p in parts[1:]:
+            out += [sl.mutate(unit, divergence, rng), p]
+        return np.concatenate(out)
+    return [carrier(2_000_000)], [carrier(1_000_000)], dict(repeat_copies=copies, element=element, divergence=divergence)
+
+
+def run_group_sizes(name, targets, queries, steps, warmup, extra, sizes, seed="12of19", max_word_count=0):
     """Default mode at each group size in `sizes`, the runs alternating; asserts that every size gives the first's output."""
     from genomeworks_b200 import cudaextender as ce
-    aligners = {g: ce.GenomeAligner(group_bases=g) for g in sizes}
+    aligners = {g: ce.GenomeAligner(group_bases=g, seed=seed, max_word_count=max_word_count) for g in sizes}
     for _ in range(warmup):
         for al in aligners.values():
             al.run(targets, queries)
@@ -123,16 +148,19 @@ def run_group_sizes(name, targets, queries, steps, warmup, extra, sizes):
         same = bool(np.array_equal(out[g][0], first[0]) and out[g][1] == first[1])
         assert same, "group_bases %d changed the output" % g
         ms, counts = al.last_stats()
-        more = dict(extra, mode="default", group_bases=g, group_stats=al.last_group_stats(), target_records=len(targets),
+        more = dict(extra, mode="default", group_bases=g, seed=seed, max_word_count=max_word_count, group_stats=al.last_group_stats(),
+                    target_records=len(targets),
                     query_records=len(queries), same_output_as_group_bases=sizes[0] if len(sizes) > 1 else None)
         al.close()
         line(name, targets, queries, steps, warmup, out[g][0], wall[g], ms, counts, more)
 
 
-def run(name, targets, queries, steps, warmup, extra, modes=("default",), min_chain_score=30000, placed=None, group_bases=1 << 28):
+def run(name, targets, queries, steps, warmup, extra, modes=("default",), min_chain_score=30000, placed=None, group_bases=1 << 28,
+        seed="12of19", max_word_count=0):
     from genomeworks_b200 import cudaextender as ce
     aligners = {m: ce.GenomeAligner(skip_covered=m.endswith("skip"), chain=m.startswith("chain"),
-                                    min_chain_score=min_chain_score if m.startswith("chains") else None, group_bases=group_bases)
+                                    min_chain_score=min_chain_score if m.startswith("chains") else None, group_bases=group_bases,
+                                    seed=seed, max_word_count=max_word_count)
                 for m in modes}
     for _ in range(warmup):
         for al in aligners.values():
@@ -146,7 +174,7 @@ def run(name, targets, queries, steps, warmup, extra, modes=("default",), min_ch
             wall[m] += (time.perf_counter() - t0) / steps
     for m, al in aligners.items():
         ms, counts = al.last_stats()
-        more = dict(extra, mode=m, group_bases=group_bases, group_stats=al.last_group_stats())
+        more = dict(extra, mode=m, group_bases=group_bases, seed=seed, max_word_count=max_word_count, group_stats=al.last_group_stats())
         if m.startswith("chain"):
             more["chain_stats"] = al.last_chain_stats()
             more["chains"] = al.last_chain_count()
@@ -188,10 +216,16 @@ def main():
     ap.add_argument("--min-chain-score", type=int, default=30000)
     ap.add_argument("--group-bases", type=int, default=1 << 28)
     ap.add_argument("--contigs", type=int, default=2000)
+    ap.add_argument("--seed", default="12of19")
+    ap.add_argument("--max-word-count", type=int, default=0)
+    ap.add_argument("--repeat-copies", type=int, default=300)
     a = ap.parse_args()
     modes = ["skip"] if a.skip_covered else a.modes.split(",")
     if set(modes) - {"default", "skip", "chain", "chain+skip", "chains", "chains+skip"}:
         sys.exit("modes are default, skip, chain, chain+skip, chains and chains+skip")
+    from genomeworks_b200 import cudaextender as ce
+    ce._seed_args(a.seed, a.max_word_count)
+    seeding = dict(seed=a.seed, max_word_count=a.max_word_count)
     import torch
     if not torch.cuda.is_available():
         sys.exit("bench_genome_aligner.py needs a CUDA device")
@@ -199,17 +233,20 @@ def main():
         if w == "sample":
             import extender_libs as xl
             seq, _, _ = xl.sample()
-            run("sample", [seq], [seq], a.steps, a.warmup, {}, modes, a.min_chain_score, group_bases=a.group_bases)
+            run("sample", [seq], [seq], a.steps, a.warmup, {}, modes, a.min_chain_score, group_bases=a.group_bases, **seeding)
         elif w == "assembly":
             t, q, extra, placed = assembly()
-            run("assembly", t, q, a.steps, a.warmup, extra, modes, a.min_chain_score, placed, a.group_bases)
+            run("assembly", t, q, a.steps, a.warmup, extra, modes, a.min_chain_score, placed, a.group_bases, **seeding)
         elif w == "contigs":
             t, q, extra, placed = assembly()
             rng = np.random.default_rng(7)
             targets = cut(t[0], a.contigs, rng)
             pieces = [q[0][qb:qe] for qb, qe, _, _, _ in placed]
-            run_group_sizes("contigs_x_pieces", targets, pieces, a.steps, a.warmup, extra, [a.group_bases, 1])
-            run_group_sizes("contigs_x_contigs", targets, cut(q[0], a.contigs, rng), a.steps, a.warmup, extra, [a.group_bases])
+            run_group_sizes("contigs_x_pieces", targets, pieces, a.steps, a.warmup, extra, [a.group_bases, 1], **seeding)
+            run_group_sizes("contigs_x_contigs", targets, cut(q[0], a.contigs, rng), a.steps, a.warmup, extra, [a.group_bases], **seeding)
+        elif w == "repeats":
+            t, q, extra = repeats(a.repeat_copies)
+            run("repeats", t, q, a.steps, a.warmup, extra, modes, a.min_chain_score, group_bases=a.group_bases, **seeding)
         else:
             sys.exit("unknown workload " + w)
 

@@ -33,8 +33,13 @@ namespace
      options:
         -s, --strand
             plus, minus or both [both]; minus aligns the query's reverse complement and reports forward query coordinates
+        --seed
+            the spaced seed: 12of19, 14of22, match<N> (N consecutive care positions, N = 1 ... 14), or a pattern of 1 (care)
+            and 0 (don't care) with a 1 at both ends, span 1 to 32 and 1 to 14 care positions [12of19]
+        --max-word-count=N
+            drop the hits of a seed word that occurs more than N times over all target records (0: no cap) [0]
         --no-transition
-            seed with exact 12-of-19 hits only (default: one transition allowed at a care position)
+            seed with exact hits only (default: one transition allowed at a care position)
         -x, --xdrop
             X-drop of the ungapped extension [910]
         -T, --ssp-threshold
@@ -152,6 +157,7 @@ int main(int argc, char* argv[])
         {"block-size", required_argument, 0, 'B'},      {"traceback-budget", required_argument, 0, 'b'},
         {"skip-covered", no_argument, 0, 257},          {"chain", optional_argument, 0, 258},
         {"chain-min-score", required_argument, 0, 259}, {"group-bases", required_argument, 0, 260},
+        {"seed", required_argument, 0, 261},            {"max-word-count", required_argument, 0, 262},
         {"version", no_argument, 0, 'v'},               {"help", no_argument, 0, 'h'},
         {0, 0, 0, 0},
     };
@@ -162,6 +168,8 @@ int main(int argc, char* argv[])
     int32_t chain_pen[2] = {0, 0};
     int64_t chain_min    = 0;
     int64_t group_bases  = int64_t(1) << 28;
+    std::string seed     = "12of19";
+    int64_t max_words    = 0;
     int argument      = 0;
     while ((argument = getopt_long(argc, argv, "s:x:T:y:o:e:g:B:b:vh", options, nullptr)) != -1)
     {
@@ -206,6 +214,18 @@ int main(int argc, char* argv[])
             chain_min = to_int(optarg, "chain-min-score", INT64_MIN, INT64_MAX);
             break;
         case 260: group_bases = to_int(optarg, "group-bases", 1, i32); break;
+        case 261:
+            seed = optarg;
+            // the pattern is checked before the handle is looked at
+            if (gwb200_genome_aligner_set_seed(nullptr, seed.c_str(), 0) == GWB200_EXT_INVALID_INPUT)
+            {
+                std::cerr << "ERROR: seed must be 12of19, 14of22, match<N> (N = 1 ... 14) or a pattern of 0 and 1 with a 1 at both ends, "
+                             "span 1 to 32 and 1 to 14 care positions, not '"
+                          << seed << "'" << std::endl;
+                std::exit(1);
+            }
+            break;
+        case 262: max_words = to_int(optarg, "max-word-count", 0, INT64_MAX); break;
         case 'x': p.xdrop = static_cast<int32_t>(to_int(optarg, "xdrop", 0, i32)); break;
         case 'T': p.ssp_threshold = static_cast<int32_t>(to_int(optarg, "ssp-threshold", -i32 - 1, i32)); break;
         case 'y': p.ydrop = static_cast<int32_t>(to_int(optarg, "ydrop", 0, 1 << 28)); break;
@@ -247,6 +267,8 @@ int main(int argc, char* argv[])
         fail("could not set the minimum chain score");
     if (gwb200_genome_aligner_set_group_bases(a, group_bases) != 0)
         fail("could not set the group size");
+    if (gwb200_genome_aligner_set_seed(a, seed.c_str(), max_words) != 0)
+        fail("could not set the seed");
     const int rc = gwb200_genome_aligner_run(a, tcodes.data(), toff.data(), static_cast<int32_t>(targets.size()), qcodes.data(), qoff.data(),
                                              static_cast<int32_t>(queries.size()));
     if (rc != 0)
